@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""bench.py -- the hot path's benchmark (contract: task brief §④).
+"""bench.py -- the hot path's benchmark.
 
 One "step" = one DIR training step on one synthetic batch per GPU:
   ResNet-50 forward (train-mode BN) -> FDS.smooth (live tables, epoch >= 2 state)
@@ -35,7 +35,7 @@ WORKLOAD = "IMDB-WIKI-DIR ResNet-50 + FDS (feature_dim 2048, bucket_num 100, buc
 BUCKET_NUM, BUCKET_START = 100, 0
 FWD_GFLOP_PER_IMG = 8.174          # SURVEY.md §8(d)
 FWDBWD_GFLOP_PER_IMG = 24.29
-SPEC_BF16_TFLOPS = 2250.0          # B200 dense bf16, nominal (B200_PROFILING.md)
+SPEC_BF16_TFLOPS = 989.0           # H100 SXM dense bf16, NVIDIA data sheet (700 W card)
 
 
 def measured_peaks():
@@ -44,7 +44,7 @@ def measured_peaks():
         d = json.load(open(path))
         return dict(hbm_gbs=d["hbm_gbs"], bf16_burst=d["bf16_tflops"], bf16_sustained=d["bf16_tflops_sustained"],
                     source="measured (MEASURED_PEAKS.json)")
-    return dict(hbm_gbs=6650.0, bf16_burst=1590.0, bf16_sustained=1400.0, source="fallback (B200_PROFILING.md)")
+    return dict(hbm_gbs=3350.0, bf16_burst=989.0, bf16_sustained=989.0, source="H100 SXM data sheet (not measured)")
 
 
 class ClockSampler:
@@ -103,7 +103,7 @@ def synthetic_labels(n, seed):
 # ----------------------------------------------------------------------------- CPU arm
 def cpu_threads():
     """Host threads for the CPU arm: all cores up to 32 -- beyond that torch's CPU conv/BN kernels on a small batch
-    slow down badly (measured on the 128-thread B200 host: 0.05-0.5 img/s with 128 threads)."""
+    slow down badly (0.05-0.5 img/s with 128 threads on a 128-thread host)."""
     return max(1, min(os.cpu_count() or 1, 32))
 
 
@@ -115,7 +115,7 @@ def _epoch_features(n=12208, seed=7):
 
 
 class _CpuArm:
-    """The reference's own modules (baseline/_ref, oracle/ref_step.py) when installed, else the port
+    """The reference's own modules (oracle/_ref, oracle/ref_step.py) when installed, else the port
     (oracle/train_ref.py); same step either way: ResNet-50 fwd (train-mode BN) -> FDS.smooth (epoch >= 2 tables) ->
     regressor -> LDS-weighted L1 -> backward -> Adam, fp32 on the host cores."""
 
@@ -128,7 +128,7 @@ class _CpuArm:
             self.kind = "reference"
             self.tr = ref_step.ReferenceTrainer(bucket_num=BUCKET_NUM, bucket_start=BUCKET_START, epoch_features=feats,
                                                 epoch_labels=lab)
-            self.what = "the reference's own resnet.py / fds.py / loss.py (baseline/_ref), torch fp32 CPU kernels"
+            self.what = "the reference's own resnet.py / fds.py / loss.py (oracle/_ref), torch fp32 CPU kernels"
         else:
             from oracle.train_ref import RefTrainer
             self.kind = "port"
@@ -137,7 +137,7 @@ class _CpuArm:
             tables = (torch.randn(nb, 2048, generator=g) * .1 + .5, torch.rand(nb, 2048, generator=g) + .5,
                       torch.randn(nb, 2048, generator=g) * .1 + .5, torch.rand(nb, 2048, generator=g) + .5)
             self.tr = RefTrainer(bucket_num=BUCKET_NUM, bucket_start=BUCKET_START, fds_tables=tables)
-            self.what = "oracle/train_ref.py (port: baseline/_ref not installed), torch fp32 CPU kernels"
+            self.what = "oracle/train_ref.py (port: oracle/_ref not installed), torch fp32 CPU kernels"
 
     def batch(self, bs):
         g = torch.Generator().manual_seed(0)
@@ -264,14 +264,32 @@ def make_batches(args, device, rank, ep_labels, w_all, pinned):
 
 
 def train_step(model, opt, x, t, w, epoch=2):
+    """One training step; returns (predictions, smoothed features, loss) as a caller of the step receives them."""
     from loss import weighted_l1_loss
-    outputs, _ = model(x, t, epoch)
+    outputs, feats = model(x, t, epoch)
     loss = weighted_l1_loss(outputs, t, w)
     opt.zero_grad()
     loss.backward()
     model.reduce_gradients()
     opt.step()
-    return loss
+    return outputs, feats, loss
+
+
+DUMP_SAMPLE = 1 << 20      # parameters / gradients: a fixed, seeded sample of this many entries of the flat buffers
+
+
+def dump_outputs(directory, model, outputs, feats, loss):
+    """The last timed step's predictions, features and loss, and a fixed seeded sample (indices stored alongside) of
+    the updated parameters and applied gradients, as .npy files (~19 MB)."""
+    os.makedirs(directory, exist_ok=True)
+    flat_p, flat_g = model.module.flat_parameters(), model.module.flat_grads()
+    idx = np.sort(np.random.RandomState(0).choice(flat_p.numel(), size=min(DUMP_SAMPLE, flat_p.numel()), replace=False))
+    sel = torch.from_numpy(idx).to(flat_p.device)
+    arrays = {"pred": outputs, "features": feats, "loss": loss.reshape(1), "params_sample": flat_p[sel],
+              "grads_sample": flat_g[sel]}
+    for name, a in arrays.items():
+        np.save(os.path.join(directory, name + ".npy"), a.detach().float().cpu().numpy())
+    np.save(os.path.join(directory, "sample_index.npy"), idx.astype(np.float64))
 
 
 def timed(fn, steps, warmup, world, device):
@@ -427,9 +445,10 @@ def run_ours(args):
 
     # ---- (1) device-resident throughput: `value`
     dev_batches = make_batches(args, device, rank, ep_labels, w_all, pinned=False)
+    last = {}
     def step_resident(i):
         x, t, w = dev_batches[i % len(dev_batches)]
-        train_step(model, opt, x, t, w)
+        last["out"] = train_step(model, opt, x, t, w)
     sampler = ClockSampler(local)
     timed(step_resident, 0, args.warmup, world, device)
     launches0 = _lib.launch_count()
@@ -439,6 +458,8 @@ def run_ours(args):
     launches = _lib.launch_count() - launches0
     ms_per_step = dev_ms / args.steps
     value = world * args.batch * args.steps / (dev_ms / 1e3)
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, model, *last["out"])
 
     # ---- (2) end to end: pinned host batches, H2D every step (prefetched on a side stream), loss read back
     host_batches = make_batches(args, device, rank, ep_labels, w_all, pinned=True)
@@ -458,7 +479,7 @@ def run_ours(args):
         (x, t, w), ev = slots[i % 2]
         torch.cuda.current_stream().wait_event(ev)
         prefetch(i + 1)
-        loss = train_step(model, opt, x, t, w)
+        loss = train_step(model, opt, x, t, w)[2]
         for a in (x, t, w):
             a.record_stream(torch.cuda.current_stream())
         if loss_events[i % 2] is not None:
@@ -481,18 +502,11 @@ def run_ours(args):
     f, d, wg = conv_flops_per_image()
     conv_ms = prof["conv_fprop"][0] + prof["conv_dgrad"][0] + prof["conv_wgrad"][0]
     conv_flops = (f + d + wg) * args.batch
-    # DRAM traffic of the same kernels from the committed ncu launch list (profiles/r2_launches.json: sum of
-    # dram__bytes_read + dram__bytes_write over the conv launches of one step), else null
-    traffic = None
-    tpath = os.path.join(ROOT, "profiles", "r2_launches.json")
-    if os.path.exists(tpath) and args.batch == 256:
-        traffic = json.load(open(tpath)).get("conv_dram_gb")
     nlaunch = prof['conv_fprop'][1] + prof['conv_dgrad'][1] + prof['conv_wgrad'][1]
-    roofline = {"bound": "tensor", "kernel": "igemm_kernel (tcgen05 implicit-GEMM conv: fprop+dgrad+wgrad, "
+    roofline = {"bound": "tensor", "kernel": "igemm_kernel (wgmma implicit-GEMM conv: fprop+dgrad+wgrad, "
                 f"{nlaunch} launch groups/step; achieved = their summed algorithmic FLOPs / summed CUDA-event time)",
                 "achieved": conv_flops / (conv_ms / 1e3) / 1e12, "peak": peaks["bf16_sustained"], "unit": "TFLOP/s",
-                "frac": conv_flops / (conv_ms / 1e3) / 1e12 / peaks["bf16_sustained"], "traffic": traffic,
-                "traffic_unit": "GB of DRAM read+write per step over these launches (ncu)",
+                "frac": conv_flops / (conv_ms / 1e3) / 1e12 / peaks["bf16_sustained"],
                 "peak_source": peaks["source"] + ", sustained (kernel timed inside a long step)",
                 "algorithmic_gflop_per_step": conv_flops / 1e9, "kernel_ms_per_step": conv_ms,
                 "note": "the timed launches also do BatchNorm work in their epilogues (fprop: batch statistics of its "
@@ -523,7 +537,7 @@ def run_ours(args):
                "warmup": args.warmup, "ms_per_step": ms_per_step, "higher_is_better": True, "scaling": "weak",
                "vs_baseline": None, "dtype": "bf16", "data": "synthetic",
                "config": {"workload": WORKLOAD, "batch_per_gpu": args.batch, "global_batch": args.batch * world,
-                          "parallelism": f"dp{world}", "l2": "per-step working set (~11 GB of activations) >> 126 MB L2; "
+                          "parallelism": f"dp{world}", "l2": "per-step working set (~11 GB of activations) >> 50 MB L2; "
                           f"{args.num_batches} distinct input batches", "timing": "CUDA events, max over ranks"},
                "e2e": {"value": e2e_value, "unit": "images/s", "h2d_bytes_per_step": h2d, "d2h_bytes_per_step": 4,
                        "ms_per_step": max(e2e_dev_ms, e2e_wall_ms) / args.steps},
@@ -538,7 +552,8 @@ def run_ours(args):
                "kernel_breakdown_note": "from 2 extra profiling-mode steps (CUDA events around every launch group: "
                                         "their sum exceeds ms_per_step by the event overhead); not part of the timed steps",
                "model_flops_utilisation": FWDBWD_GFLOP_PER_IMG * args.batch / ms_per_step / SPEC_BF16_TFLOPS,
-               "model_flops_utilisation_note": "24.29 GFLOP/img fwd+bwd vs the nominal dense bf16 peak (2250 TFLOP/s)",
+               "model_flops_utilisation_note": "24.29 GFLOP/img fwd+bwd vs the H100 SXM data-sheet dense bf16 peak "
+                                               "(989 TFLOP/s at 700 W)",
                "step_frac_of_measured_bf16_peak": FWDBWD_GFLOP_PER_IMG * args.batch / ms_per_step / peaks["bf16_sustained"],
                "replica_check": replica_check}
         sys.stdout.flush()
@@ -559,7 +574,11 @@ def main():
     ap.add_argument("--cpu-batch", dest="cpu_batch", type=int, default=16,
                     help="images per step of the CPU arm (a bounded sample of the 256-image step)")
     ap.add_argument("--no-cpu-baseline", dest="no_cpu_baseline", action="store_true")
+    ap.add_argument("--dump-outputs", dest="dump_outputs", metavar="DIR", default=None,
+                    help="write what the last timed step computed to DIR/<name>.npy (float32)")
     args = ap.parse_args()
+    if args.dump_outputs and args.impl != "ours":
+        ap.error("--dump-outputs writes the outputs of the GPU arm's timed step; it does not apply to --impl reference")
     args.warmup = max(args.warmup, 3) if args.impl == "ours" else args.warmup
     if args.impl == "reference":
         run_reference(args)

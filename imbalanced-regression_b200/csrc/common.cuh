@@ -1,4 +1,4 @@
-// Shared host/device helpers for libdirb200 (sm_100a only).
+// Shared host/device helpers for libdirb200 (sm_90a only).
 #pragma once
 #include <cuda_runtime.h>
 #include <cuda_bf16.h>
@@ -46,8 +46,8 @@ inline int num_sms() {
   static int n = 0;
   if (n == 0) {
     int dev = 0;
-    if (cudaGetDevice(&dev) != cudaSuccess) return 148;
-    if (cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || n <= 0) n = 148;
+    if (cudaGetDevice(&dev) != cudaSuccess) return 132;
+    if (cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || n <= 0) n = 132;
     if (const char* e = getenv("DIRB200_SMS")) {
       const int cap = atoi(e);
       if (cap > 0 && cap < n) n = cap;
@@ -67,9 +67,8 @@ __device__ __forceinline__ double warp_sum(double v) {
   return v;
 }
 
-// Division by a run-time constant as multiply-high + shift (n < 2^31, d >= 1): the k-loops of the producer / TMA
-// warps used to spend most of their time in the ~35-instruction SASS sequences of `/` by cpb, kw, hw, wm
-// (ncu source page, profiles/r2_conv_stalls.md) -- that, not the memory system, was the "gather rate".
+// Division by a run-time constant as multiply-high + shift (n < 2^31, d >= 1): a 32-bit `/` by a run-time divisor
+// (cpb, kw, hw, wm) compiles to a ~35-instruction SASS sequence, which would dominate the k-loops of the producer warps.
 struct FastDiv {
   uint32_t mul, shr, d;
   __device__ __forceinline__ uint32_t div(uint32_t n) const { return d == 1 ? n : (__umulhi(n, mul) >> shr); }

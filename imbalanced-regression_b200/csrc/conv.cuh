@@ -8,8 +8,8 @@ struct ConvShape {
   int n, h, w, cin, cout, kh, kw, stride, pad, ho, wo;
 };
 
-// Which rows of a per-CTA statistics buffer [rows][2][c] hold the partial sums of a channel: the CTAs (or CTA pairs,
-// group = 2) are dealt round-robin over the n_tiles column tiles of width bn, so channel ch lives in the rows
+// Which rows of a per-CTA statistics buffer [rows][2][c] hold the partial sums of a channel: the CTAs (or groups of
+// `group` CTAs) are dealt round-robin over the n_tiles column tiles of width bn, so channel ch lives in the rows
 // (j + k * n_tiles) * group + r   with j = ch / bn, k = 0 .. while the row index < rows, r = 0 .. group-1.
 // A plain column reduction over all rows is {rows, 1, c, 1}.
 struct StatLayout {

@@ -1,5 +1,5 @@
 // C-ABI entry points of the convolution stage + the small layout kernels around
-// the tcgen05 implicit GEMM (weight re-layout, stem space-to-depth, split-K reduce).
+// the wgmma implicit GEMM (weight re-layout, stem space-to-depth, split-K reduce).
 #include "common.cuh"
 #include "conv.cuh"
 
@@ -310,9 +310,9 @@ int dirb200_conv_wgrad(const void* x, const void* dy, float* dw, void* workspace
 }
 
 /* Host-only (no CUDA call): the GEMM form dirb200_conv_fprop / _dgrad / _wgrad (op 0 / 1 / 2) would launch for this
- * shape: plan7[0] tile width BN, [1] CTA pairs, [2] A-operand form (0 cp.async gather, 1 tiled TMA, 2 im2col TMA, 3
- * patch-resident), [3] image rows per tile of the patch form, [4] split-K factor, [5] launches, [6] dgrad can carry the
- * BN-backward moments of the previous layer. */
+ * shape: plan7[0] tile width BN, [1] 0 (no CTA pairs), [2] A-operand form (0 cp.async gather, 1 tiled TMA, 2 im2col
+ * TMA), [3] 0 (no patch-resident form), [4] split-K factor, [5] launches, [6] dgrad can carry the BN-backward moments of
+ * the previous layer. */
 int dirb200_conv_plan(int n, int h, int w, int cin, int cout, int kh, int kw, int stride, int pad, int stem, int op,
                       int* plan7) {
   DIRB_CHECK_ARG(plan7 && op >= 0 && op <= 2, "conv_plan: bad arguments");

@@ -1,16 +1,11 @@
-// Implicit-GEMM convolution on the 5th-gen tensor cores (tcgen05 + TMEM + TMA),
+// Implicit-GEMM convolution on the Hopper tensor cores (wgmma + TMA + mbarrier),
 // NHWC bf16 activations, fp32 accumulation.  Stage (i) of the hot path:
 // replaces the cuDNN convolutions behind agedb-dir/resnet.py:46-51,79,112-118
 // (forward) and their autograd backward (data and weight gradients).
 //
-// Persistent kernel: one CTA per SM walks the 128 x BN output tiles round-robin; the smem ring and the two
-// TMEM accumulators run across tile boundaries, so loads, MMAs and epilogues of neighbouring tiles overlap:
-//   warps 0-3  gather the A operand (im2col rows) global -> swizzled smem with 16-byte cp.async
-//              (zero-fill = padding) -- idle when A is a plain matrix (1x1 stride-1 convs) or im2col TMA is on;
-//   warp 4     streams the B operand (weights, or dY for wgrad) with TMA, and the A operand in the TMA-fed forms;
-//   warp 5     owns TMEM and issues tcgen05.mma (warp converged, one elected lane issues);
-//   warps 6-9  epilogue: tcgen05.ld TMEM -> registers -> global, then hand the accumulator back.
-// mbarriers: full/empty per smem stage, full/empty per TMEM accumulator.
+// Persistent kernel: one CTA per SM walks the 128 x BN output tiles; the smem ring (full / empty mbarrier per stage)
+// runs across tile boundaries.  Warpgroup 0 produces (cp.async gather of A + TMA of B, or TMA of both); warpgroups 1
+// and 2 consume rows [0, 64) / [64, 128) of the tile with wgmma, accumulators in registers, epilogue from registers.
 //
 //   FPROP  Y[p, co]  = sum_k  A[p, k] W[co, k]      A, W K-major      (k = (r, s, c))
 //   DGRAD  dX[p, c]  = sum_k  A'[p, k] Wt[c, k]     same kernel, transposed gather (k = (r, s, co))
@@ -25,10 +20,10 @@ using namespace tc;
 
 constexpr int BM = 128;  // GEMM rows per tile (pixels; for wgrad: 2 chunks x 64 gathered channels)
 constexpr int BK = 64;   // bf16 elements per k-block = one 128-byte swizzle row
-constexpr int kProducerThreads = 128;   // warps 0-3
-constexpr int kTmaWarp = 4, kMmaWarp = 5; // warps 6-9: epilogue (warp & 3 = TMEM lane quarter)
-constexpr int kThreads = 320;
+constexpr int kProducerThreads = 128;   // warpgroup 0
+constexpr int kThreads = 384;           // + two consumer warpgroups
 constexpr int kMaxTaps = 25;   // up to 5x5 filters (the NYUD2 decoder / refinement convs, nyud2-dir/models/modules.py:11-20,154-160)
+constexpr int kMaxSmemBytes = 232448;   // opt-in shared memory per block (227 KB)
 
 struct IgemmParams {
   const __nv_bfloat16* src;  // gathered tensor, NHWC
@@ -57,9 +52,9 @@ struct IgemmParams {
   int a_mode;                // ATMA kernels: 1 = A is a plain [pixels][channels] matrix (tiled TMA), 2 = im2col TMA
   int i2c_stride, i2c_lo;    // im2col: base pixel of GEMM row (y, x) = (y * i2c_stride + i2c_lo, x * i2c_stride + i2c_lo)
   int ldc;                   // output row stride in elements (Cout for fprop, Cin for dgrad, Cout for wgrad partials)
-  void* out;                 // bf16 [pixels][ldc]   or   fp32 [splits][total_chunks*64][ldc]
+  void* out;                 // bf16 [pixels][ldc]   or   fp32 [splits][Cout][total_chunks*64]
   // fprop only, optional: per-column sum / sum of squares of the (bf16-rounded) output = the BatchNorm batch
-  // statistics of the layer, carried in the epilogue warps' registers over all tiles of the CTA and written once per
+  // statistics of the layer, carried in per-warp shared-memory slots over all tiles of the CTA and written once per
   // CTA as stat_out[blockIdx.x][2][ldc] (fp32), columns [n_tile * BN, n_tile * BN + BN) of the CTA's fixed n_tile only
   // (see StatLayout for which rows hold which columns)
   float* stat_out;
@@ -76,48 +71,25 @@ struct IgemmParams {
   const __nv_bfloat16* bst_y;
   const float* bst_scale;
   const float* bst_shift;
-  // PATCH kernels (3x3 / stride 1 / pad 1, 64 -> 64 channels): a GEMM tile is `patch_r` whole image rows in PADDED
-  // coordinates (row m of the tile = (yy, xx) = divmod(m, patch_wp), patch_wp = W + 2; rows with xx >= W or yy >= patch_r
-  // are dead), its A operand ONE (patch_r + 2) x patch_wp x 64-channel input patch that stays in shared memory for all
-  // nine taps: tap (r, s) reads it displaced by r * patch_wp + s rows (dgrad, `transposed`: (2 - r) * patch_wp + 2 - s).
-  int patch_r, patch_wp, patch_h, patch_w;
-  FastDiv fd_tpi, fd_wp;       // tiles per image (H / patch_r), patch_wp
 };
 
-// CTA2: the tile is computed by a CTA pair (cta_group::2, UMMA M = 256): this CTA owns 128 of the 256 rows and stages
-// only HALF of the B tile (BN/2 rows) -- 1/3 less L2->smem operand traffic per FLOP at BN = 256.
-template <int BN, bool STAGED_EPI, bool CTA2 = false, bool PATCH = false>
+template <int BN, bool STAGED_EPI>
 struct Cfg {
   static constexpr int kABytes = BM * BK * 2;
-  static constexpr int kBRows = CTA2 ? BN / 2 : BN;      // B rows staged by this CTA
-  static constexpr int kBBytes = kBRows * BK * 2;
-  // PATCH: a ring stage (3 of them) is one input patch (<= 32 KB incl. the rows the last taps read past its end); the nine weight
-  // k-blocks are loaded once per CTA and stay resident behind the ring
-  static constexpr int kStageBytes = PATCH ? 32768 : kABytes + kBBytes;
-  static constexpr int kBresBytes = PATCH ? 9 * BN * BK * 2 : 0;
-  // smem: operand ring + (fprop/dgrad) a per-epilogue-warp staging tile of 32 rows x kEpiCols columns, so output
-  // rows leave as whole 128-byte lines (the tile's BN columns are drained in BN / kEpiCols passes; the narrow
-  // staging buffer buys one to two more ring stages than a full-width one); one persistent CTA per SM
-  static constexpr int kEpiCols = 64;
-  static constexpr int kStages = PATCH ? 3
-                                 : CTA2 ? ((BN == 256) ? 6 : 8)
-                                        : (STAGED_EPI ? ((BN == 256) ? 4 : ((BN == 128) ? 6 : 8))
-                                                      : ((BN == 256) ? 4 : ((BN == 128) ? 6 : 8)));
-  static constexpr int kBresOffset = kStages * kStageBytes;
-  static constexpr int kBarOffset = kBresOffset + kBresBytes;
-  static constexpr int kStageRowBytes = kEpiCols * 2 + 16;      // +16 B: conflict-free 16-byte column writes
-  static constexpr int kEpiWarpBytes = 32 * kStageRowBytes;
-  static constexpr int kEpiOffset = kBarOffset + 256;           // after the mbarriers ((2*kStages + 6) * 8 <= 176 B)
-  // per epilogue warp: [BN / kEpiCols passes][4 (sum c0, sum c1, sumsq c0, sumsq c1)][32 lanes] fp32 running column sums
-  // of the BN statistics (kept in smem, not registers, so that the column-pass loop stays rolled: unrolled four-fold
-  // the epilogue outgrew the instruction cache and the epilogue-bound 1x1 layers lost 25 %)
-  static constexpr int kStatWarpBytes = (BN / kEpiCols) * 4 * 32 * 4;
-  // PATCH: two epilogue groups (warps 6-9 drain accumulator 0, warps 0-3 -- idle gather warps otherwise -- accumulator
-  // 1): with one input patch per tile the mainloop of a 128 x 64 tile is shorter than one group's epilogue
-  static constexpr int kEpiWarps = PATCH ? 8 : 4;
-  static constexpr int kStatOffset = kEpiOffset + (STAGED_EPI ? kEpiWarps * kEpiWarpBytes : 0);
-  static constexpr int kSmemBytes = kStatOffset + (STAGED_EPI ? kEpiWarps * kStatWarpBytes : 0) + 1024;
-  static constexpr int kTmemCols = 2 * BN;  // two accumulators (epilogue of tile i overlaps the MMAs of tile i+1)
+  static constexpr int kBBytes = BN * BK * 2;
+  static constexpr int kStageBytes = kABytes + kBBytes;
+  // as many ring stages as fit next to the epilogue buffers; one persistent CTA per SM
+  static constexpr int kStages = BN == 128 ? (STAGED_EPI ? 5 : 6) : 8;
+  static constexpr int kBarOffset = kStages * kStageBytes;
+  // fprop / dgrad: a per-consumer-warp staging tile of 16 rows x BN bf16 (+16 B per row: conflict-free fragment writes)
+  static constexpr int kStageRowBytes = BN * 2 + 16;
+  static constexpr int kEpiWarpBytes = 16 * kStageRowBytes;
+  static constexpr int kEpiOffset = kBarOffset + 256;           // after the mbarriers (2 * kStages * 8 <= 128 B)
+  // per consumer warp: [2 (sum, sum of squares)][BN] fp32 running column sums of the BN statistics
+  static constexpr int kStatWarpBytes = 2 * BN * 4;
+  static constexpr int kStatOffset = kEpiOffset + (STAGED_EPI ? 8 * kEpiWarpBytes : 0);
+  static constexpr int kSmemBytes = kStatOffset + (STAGED_EPI ? 8 * kStatWarpBytes : 0) + 1024;
+  static_assert(kSmemBytes <= kMaxSmemBytes, "shared memory budget");
 };
 
 // ---- A-operand gather --------------------------------------------------------------------------------
@@ -182,69 +154,45 @@ __device__ __forceinline__ const __nv_bfloat16* tap_source(const IgemmParams& P,
        static_cast<unsigned>(wi) < static_cast<unsigned>(P.ws);
   return ok ? P.src + (static_cast<size_t>(rp.nb + hi) * P.ws + wi) * P.cs + coff : P.src;
 }
-
-// CTA2 (fprop / stride-1 dgrad, BN = 256, TMA-fed A operand): launched as (2,1,1) clusters; the pair owns a 256 x 256
-// tile.  Per k-block each CTA TMA-loads its own 128 A rows and its half of B with .cta_group::2 loads whose bytes are
-// all counted on the LEADER's full barrier (one expect_tx arrival by the leader's TMA warp); the leader issues
-// tcgen05.mma.cta_group::2 and its commits arrive on the empty / accumulator-full barriers of both CTAs (multicast);
-// the peer's epilogue warps hand the accumulator back by arriving on the leader's barrier.
-//
 // ATMA: the A operand comes by TMA -- tiled maps for 1x1 / stride-1 convolutions (a plain [pixels][channels] matrix:
 // K-major 64 x 128 boxes for fprop / dgrad, two 64 x 64 MN-major boxes for wgrad), im2col-mode maps for the 3x3 and
-// strided ones -- issued by warp 4; warps 0-3 then idle.  Without ATMA (stem, stride-2 dgrad parity classes) warps 0-3
-// gather the rows with cp.async.
-template <int BN, bool WGRAD, bool STEM, bool CTA2 = false, bool ATMA = false, bool AFFINE = false, bool BSTAT = false,
-          bool PATCH = false>
-__global__ void __launch_bounds__((ATMA && !PATCH) ? kThreads - kProducerThreads : kThreads, 1)
+// strided ones -- issued by warp 0.  Without ATMA (stem, or with the TMA forms switched off) warps 0-3 gather the rows
+// with cp.async.
+template <int BN, bool WGRAD, bool STEM, bool ATMA = false, bool AFFINE = false, bool BSTAT = false>
+__global__ void __launch_bounds__(kThreads, 1)
 igemm_kernel(const __grid_constant__ CUtensorMap tmap_b, const __grid_constant__ CUtensorMap tmap_a,
              const IgemmParams P) {
-  using C = Cfg<BN, !WGRAD, CTA2, PATCH>;
-  static_assert(!PATCH || (ATMA && !WGRAD && !CTA2 && !AFFINE && BN == 64), "patch-resident A operand: 64-wide fprop / dgrad");
-  static_assert(!CTA2 || (ATMA && !WGRAD && !STEM && BN >= 128), "CTA pairs: TMA-fed fprop / dgrad GEMMs only");
+  using C = Cfg<BN, !WGRAD>;
+  static_assert(BN == 64 || BN == 128, "tile width: one m64n64 / m64n128 wgmma per warpgroup and k step");
   static_assert(!ATMA || !STEM, "TMA-fed A operand: not for the stem");
   static_assert(!AFFINE || (ATMA && !WGRAD), "folded-BN epilogue: TMA-fed fprop GEMMs only");
   static_assert(!BSTAT || (ATMA && !WGRAD && !AFFINE), "BN-backward moments in the epilogue: TMA-fed dgrad GEMMs only");
   extern __shared__ uint8_t smem_raw[];
   const uint32_t smem_base = (smem_u32(smem_raw) + 1023u) & ~1023u;
+  uint8_t* const smem_gen = smem_raw + (smem_base - smem_u32(smem_raw));
   const uint32_t bar_base = smem_base + C::kBarOffset;
   auto a_addr = [&](int s) { return smem_base + s * C::kStageBytes; };
   auto b_addr = [&](int s) { return smem_base + s * C::kStageBytes + C::kABytes; };
   constexpr uint32_t nstages = C::kStages;
   auto full_bar = [&](int s) { return bar_base + 8u * s; };
   auto empty_bar = [&](int s) { return bar_base + 8u * (C::kStages + s); };
-  auto tfull_bar = [&](int a) { return bar_base + 8u * (2 * C::kStages + a); };
-  auto tempty_bar = [&](int a) { return bar_base + 8u * (2 * C::kStages + 2 + a); };
-  const uint32_t tmem_holder = bar_base + 8u * (2 * C::kStages + 4);
-  const uint32_t bres_bar = bar_base + 8u * (2 * C::kStages + 5);    // PATCH: the resident weights have landed
-  const uint32_t bres_addr = smem_base + C::kBresOffset;
-
-  // TMA-fed kernels are launched WITHOUT the four gather warps (192 threads: TMA, MMA, 4 epilogue warps; the warp
-  // numbering below keeps the roles' indices): with 10 warps a sub-partition hosts 3 of them and the register file caps
-  // a thread at 168 registers, which the epilogues with fused statistics / BN-backward moments spilled over; with 6
-  // warps (2 per sub-partition at most) the cap is 255.  warp & 3 (the TMEM lane quarter of an epilogue warp) is
-  // unchanged by the shift.
-  // (PATCH kernels keep all ten warps: the four low ones are a second epilogue group.)
-  const int warp = static_cast<int>(threadIdx.x >> 5) + ((ATMA && !PATCH) ? kProducerThreads / 32 : 0), lane = threadIdx.x & 31;
-  // CTA pair: both CTAs of a cluster walk the same sequence of pair tiles (P.m_tiles counts 256-row pair tiles)
-  const uint32_t rank = CTA2 ? cluster_ctarank() : 0u;
-  const int tile_start = CTA2 ? static_cast<int>(blockIdx.x >> 1) : static_cast<int>(blockIdx.x);
-  const int tile_stride = CTA2 ? static_cast<int>(gridDim.x >> 1) : static_cast<int>(gridDim.x);
+  const int warp = static_cast<int>(threadIdx.x >> 5), lane = threadIdx.x & 31;
 
   // Tile walk.  wgrad: work items t = (split, m_tile, n_tile) handed out round-robin (n fastest).
-  // fprop / dgrad: every CTA (pair) keeps ONE n_tile for the whole launch -- CTA c owns n = c % n_tiles and walks
+  // fprop / dgrad: every CTA keeps ONE n_tile for the whole launch -- CTA c owns n = c % n_tiles and walks
   // m = c / n_tiles, + G, + 2G, ... (G = CTAs sharing that n); neighbouring CTAs still work on the same A rows at the
-  // same time (L2 reuse), and the epilogue can carry per-column sums (BN statistics) across all of its tiles in
-  // registers and flush them once.
+  // same time (L2 reuse), and the epilogue can carry per-column sums (BN statistics) across all of its tiles and
+  // flush them once.
   int tile_first, tile_end, tile_step, fixed_n = 0;
   if constexpr (WGRAD) {
-    tile_first = tile_start; tile_end = P.num_tiles; tile_step = tile_stride;
+    tile_first = blockIdx.x; tile_end = P.num_tiles; tile_step = gridDim.x;
   } else {
     uint32_t gi, nn;
-    P.fd_ntiles.divmod(static_cast<uint32_t>(tile_start), gi, nn);
+    P.fd_ntiles.divmod(blockIdx.x, gi, nn);
     fixed_n = static_cast<int>(nn);
     tile_first = static_cast<int>(gi);
     tile_end = P.m_tiles;
-    tile_step = static_cast<int>(P.fd_ntiles.div(static_cast<uint32_t>(tile_stride - 1 - fixed_n))) + 1;
+    tile_step = static_cast<int>(P.fd_ntiles.div(gridDim.x - 1u - nn)) + 1;
   }
   auto decode_tile = [&](int t, int& split, int& m_tile, int& n_tile, int& kb_begin, int& nk) {
     if constexpr (WGRAD) {
@@ -254,48 +202,31 @@ igemm_kernel(const __grid_constant__ CUtensorMap tmap_b, const __grid_constant__
       split = static_cast<int>(sp);
       m_tile = static_cast<int>(mt);
       n_tile = static_cast<int>(nt);
-      if constexpr (CTA2) m_tile = 2 * m_tile + static_cast<int>(rank);   // this CTA's 128-row half
       kb_begin = split * P.kblocks_per_split;
       const int kb_end = min(P.num_kblocks, kb_begin + P.kblocks_per_split);
       nk = max(0, kb_end - kb_begin);
     } else {
       split = 0;
-      m_tile = CTA2 ? 2 * t + static_cast<int>(rank) : t;
+      m_tile = t;
       n_tile = fixed_n;
       kb_begin = 0;
       nk = P.num_kblocks;
     }
   };
 
-  if (warp == kMmaWarp) {
-    if (lane == 0) {
-      for (int s = 0; s < C::kStages; ++s) {
-        // TMA-fed: the TMA thread's one expect_tx arrival (pairs: everything is counted on the leader's barrier);
-        // gather-fed: + the 128 gather threads
-        mbar_init(full_bar(s), ATMA ? 1 : kProducerThreads + 1);
-        mbar_init(empty_bar(s), 1);
-      }
-      for (int a = 0; a < 2; ++a) {
-        mbar_init(tfull_bar(a), 1);
-        mbar_init(tempty_bar(a), CTA2 ? 8 : 4);      // one arrival per epilogue warp (of both CTAs of a pair)
-      }
-      if constexpr (PATCH) mbar_init(bres_bar, 1);
-      fence_barrier_init();
+  if (threadIdx.x == 0) {
+    for (int s = 0; s < C::kStages; ++s) {
+      // TMA-fed: the TMA thread's one expect_tx arrival; gather-fed: + the 128 gather threads
+      mbar_init(full_bar(s), ATMA ? 1 : kProducerThreads + 1);
+      mbar_init(empty_bar(s), 8);          // one arrival per consumer warp
     }
-    __syncwarp();
-    if constexpr (CTA2) tmem_alloc_cta2(tmem_holder, C::kTmemCols);
-    else tmem_alloc(tmem_holder, C::kTmemCols);
+    fence_barrier_init();
   }
-  tcgen05_fence_before();
-  if constexpr (CTA2) cluster_sync_all();      // the peer's barriers must be initialised before anything arrives on them
-  else __syncthreads();
-  tcgen05_fence_after();
-  uint32_t tmem_base;
-  asm volatile("ld.shared.u32 %0, [%1];" : "=r"(tmem_base) : "r"(tmem_holder));
+  __syncthreads();
 
-  if (warp < 4 && !PATCH) {
+  if (warp < 4) {
     if constexpr (!ATMA) {
-      // ============================ A producer (4 warps) ============================
+      // ===== A producer (4 warps) + B by TMA (warp 0) =====
       // Address generation is hoisted out of the k-loop: per tile each thread precomputes, for its 8 rows, the
       // element offset of the filter-tap origin and a bit mask of the taps that fall inside the image; per k-block
       // only a (warp-uniform) tap offset is added.  wgrad rows change every k-block, so there each lane resolves ONE
@@ -306,6 +237,7 @@ igemm_kernel(const __grid_constant__ CUtensorMap tmap_b, const __grid_constant__
       for (int t = tile_first; t < tile_end; t += tile_step) {
         int split, m_tile, n_tile, kb_begin, nk;
         decode_tile(t, split, m_tile, n_tile, kb_begin, nk);
+        const int n0 = n_tile * BN;
         long long off8[8];             // fprop/dgrad: origin offsets (elements) of the 8 rows this thread serves
         uint32_t mask8[8];             //              valid-tap bit masks
         int chunk_r = 0, chunk_s = 0, chunk_c0 = 0;
@@ -383,6 +315,7 @@ igemm_kernel(const __grid_constant__ CUtensorMap tmap_b, const __grid_constant__
           if (++rs == nstages) { rs = 0; rph ^= 1u; }
           const int kb = kb_begin + it;
           const uint32_t dst_base = a_addr(s) + tile_off;
+          int kcoord = kb;             // fprop/dgrad: k-block of the weight matrix
           if constexpr (!WGRAD) {
             // warp-uniform tap offset (table filled on the host; counters instead of kb / cpb, tp / kw)
             int tp;
@@ -394,6 +327,7 @@ igemm_kernel(const __grid_constant__ CUtensorMap tmap_b, const __grid_constant__
             } else {
               tp = P.tap_list[tc];
               toff = P.tap_eoff[tc] + cb * 64;
+              kcoord = tp * P.cpb + cb;
               if (++cb == P.cpb) { cb = 0; ++tc; }
             }
 #pragma unroll
@@ -428,50 +362,31 @@ igemm_kernel(const __grid_constant__ CUtensorMap tmap_b, const __grid_constant__
               const int row = 4 * i + q;                   // ... and the quarter-warp serving that row fetches it
               const unsigned long long a = __shfl_sync(0xffffffffu, rowaddr, row);
               const uint32_t okb = __shfl_sync(0xffffffffu, okbits, row);
-              bool ok;
-              const __nv_bfloat16* src;
-              if constexpr (STEM) {
-                ok = (okb >> (j >> 1)) & 1u;
-                src = reinterpret_cast<const __nv_bfloat16*>(a) + j * 8;    // 4 taps x 16 channels are contiguous
-              } else {
-                ok = okb & 1u;
-                src = reinterpret_cast<const __nv_bfloat16*>(a) + j * 8;
-              }
+              const bool ok = STEM ? ((okb >> (j >> 1)) & 1u) : (okb & 1u);
+              const __nv_bfloat16* src = reinterpret_cast<const __nv_bfloat16*>(a) + j * 8;   // stem: 4 taps x 16 channels are contiguous
               cp_async16(dst_base + row * 128 + ((j ^ (row & 7)) << 4), ok ? src : P.src, ok ? 16u : 0u);
             }
           }
+          if (warp == 0) {
+            if (elect_one()) {
+              mbar_arrive_expect_tx(full_bar(s), C::kBBytes);
+              if constexpr (!WGRAD) {
+                tma_load_2d(b_addr(s), &tmap_b, full_bar(s), kcoord * BK, n0);
+              } else {
+#pragma unroll
+                for (int i = 0; i < BN / 64; ++i)
+                  tma_load_2d(b_addr(s) + i * 8192, &tmap_b, full_bar(s), n0 + 64 * i, kb * 64);
+              }
+            }
+            __syncwarp();
+          }
           // the mbarrier receives this thread's arrival when all of its cp.async above have landed (no wait here:
-          // the ring depth alone bounds the loads in flight), as CUTLASS's sm100 cp.async->UMMA mainloop does
+          // the ring depth alone bounds the loads in flight)
           cp_async_mbar_arrive_noinc(full_bar(s));
         }
       }
-    }  // !ATMA: with a TMA-fed A operand these four warps have nothing to do
-  } else if (warp == kTmaWarp) {
-    // ============================ B producer (TMA) ============================
-    if constexpr (PATCH) {
-      // resident weights once, then one input patch per tile: (patch_r + 2) padded rows x patch_wp x 64 channels,
-      // zero-filled outside the image by the tiled TMA load (= the conv padding)
-      if (elect_one()) {
-        mbar_arrive_expect_tx(bres_bar, C::kBresBytes);
-#pragma unroll 1
-        for (int tp = 0; tp < 9; ++tp) tma_load_2d(bres_addr + tp * (BN * BK * 2), &tmap_b, bres_bar, tp * BK, 0);
-      }
-      __syncwarp();
-      const uint32_t patch_bytes = static_cast<uint32_t>((P.patch_r + 2) * P.patch_wp * 128);
-      uint32_t rs = 0, rph = 0;
-      for (int t = tile_first; t < tile_end; t += tile_step) {
-        uint32_t img, ty;
-        P.fd_tpi.divmod(static_cast<uint32_t>(t), img, ty);
-        const int s = static_cast<int>(rs);
-        mbar_wait(empty_bar(s), rph ^ 1u);
-        if (++rs == nstages) { rs = 0; rph ^= 1u; }
-        if (elect_one()) {
-          mbar_arrive_expect_tx(full_bar(s), patch_bytes);
-          tma_load_4d(a_addr(s), &tmap_a, full_bar(s), 0, -1, static_cast<int>(ty) * P.patch_r - 1, static_cast<int>(img));
-        }
-        __syncwarp();
-      }
-    } else {
+    } else if (warp == 0) {
+      // ===== A and B by TMA (warp 0) =====
       // the whole warp walks the ring (converged); one elected lane issues.  Ring position and the (tap, channel
       // block) of the k-block are counters; tap coordinates come from the host-filled tables -- no division here.
       uint32_t rs = 0, rph = 0;
@@ -480,7 +395,7 @@ igemm_kernel(const __grid_constant__ CUtensorMap tmap_b, const __grid_constant__
         decode_tile(t, split, m_tile, n_tile, kb_begin, nk);
         const int n0 = n_tile * BN;
         int tile_w0 = 0, tile_h0 = 0, tile_n0 = 0;     // im2col base pixel of the tile's first GEMM row
-        if constexpr (ATMA && !WGRAD) {
+        if constexpr (!WGRAD) {
           if (P.a_mode == 2) {
             uint32_t tn, rem, y0, x0;
             P.fd_hw.divmod(static_cast<uint32_t>(m_tile) * BM, tn, rem);
@@ -497,581 +412,232 @@ igemm_kernel(const __grid_constant__ CUtensorMap tmap_b, const __grid_constant__
           if (++rs == nstages) { rs = 0; rph ^= 1u; }
           const int kb = kb_begin + it;
           if (elect_one()) {
-            if constexpr (CTA2) {
-              // this CTA's half of the B tile; both halves are accounted on the leader's barrier
-              if (rank == 0) mbar_arrive_expect_tx(full_bar(s), 2 * (C::kBBytes + C::kABytes));
-              // ... and this CTA's 128 A rows
+            if constexpr (!WGRAD) {
+              // A tile: 128 pixel rows x 64 channels (rows past the end / padding: zeros)
+              mbar_arrive_expect_tx(full_bar(s), C::kBBytes + C::kABytes);
               if (P.a_mode == 1)
-                tma_load_2d_cta2(a_addr(s), &tmap_a, full_bar(s), kb * BK, m_tile * BM);
-              else
-                tma_load_im2col_4d_cta2(a_addr(s), &tmap_a, full_bar(s), cb * BK, tile_w0, tile_h0, tile_n0,
-                                        P.tap_s[tc], P.tap_r[tc]);
-              const int kcoord = P.tap_list[tc] * P.cpb + cb;
-              tma_load_2d_cta2(b_addr(s), &tmap_b, full_bar(s), kcoord * BK, n0 + static_cast<int>(rank) * C::kBRows);
+                tma_load_2d(a_addr(s), &tmap_a, full_bar(s), kb * BK, m_tile * BM);
+              else   // dgrad: dy pixel (y + pad - r, x + pad - s) = base + (k-1-r, k-1-s): flipped in the table
+                tma_load_im2col_4d(a_addr(s), &tmap_a, full_bar(s), cb * BK, tile_w0, tile_h0, tile_n0,
+                                   P.tap_s[tc], P.tap_r[tc]);
+              tma_load_2d(b_addr(s), &tmap_b, full_bar(s), (P.tap_list[tc] * P.cpb + cb) * BK, n0);
             } else {
-              if constexpr (ATMA) {
-                if constexpr (!WGRAD) {
-                  // A tile: 128 pixel rows x 64 channels (rows past the end / padding: zeros)
-                  mbar_arrive_expect_tx(full_bar(s), C::kBBytes + C::kABytes);
-                  if (P.a_mode == 1)
-                    tma_load_2d(a_addr(s), &tmap_a, full_bar(s), kb * BK, m_tile * BM);
-                  else   // dgrad: dy pixel (y + pad - r, x + pad - s) = base + (k-1-r, k-1-s): flipped in the table
-                    tma_load_im2col_4d(a_addr(s), &tmap_a, full_bar(s), cb * BK, tile_w0, tile_h0, tile_n0,
-                                       P.tap_s[tc], P.tap_r[tc]);
-                } else {
-                  // A tile: 64 pixels x (up to) two 64-channel chunks, MN-major like the dY tile
-                  const int nchunks = min(2, P.total_chunks - 2 * m_tile);
-                  mbar_arrive_expect_tx(full_bar(s), C::kBBytes + nchunks * 8192);
-                  if (P.a_mode == 1) {
-                    for (int i = 0; i < nchunks; ++i)
-                      tma_load_2d(a_addr(s) + i * 8192, &tmap_a, full_bar(s), (2 * m_tile + i) * 64, kb * 64);
-                  } else {
-                    // the k-block's first pixel -> base pixel; every chunk = (filter tap, 64 channels)
-                    uint32_t n0i, rem, y0, x0;
-                    P.fd_hw.divmod(static_cast<uint32_t>(kb) * 64u, n0i, rem);
-                    P.fd_wm.divmod(rem, y0, x0);
-                    for (int i = 0; i < nchunks; ++i) {
-                      uint32_t tap, cbk, r, sx;
-                      P.fd_cpb.divmod(static_cast<uint32_t>(2 * m_tile + i), tap, cbk);
-                      P.fd_kw.divmod(tap, r, sx);
-                      tma_load_im2col_4d(a_addr(s) + i * 8192, &tmap_a, full_bar(s), static_cast<int>(cbk) * 64,
-                                         static_cast<int>(x0) * P.i2c_stride + P.i2c_lo,
-                                         static_cast<int>(y0) * P.i2c_stride + P.i2c_lo, static_cast<int>(n0i),
-                                         static_cast<uint16_t>(sx), static_cast<uint16_t>(r));
-                    }
-                  }
+              // A tile: 64 pixels x (up to) two 64-channel chunks, MN-major like the dY tile
+              const int nchunks = min(2, P.total_chunks - 2 * m_tile);
+              mbar_arrive_expect_tx(full_bar(s), C::kBBytes + nchunks * 8192);
+              if (P.a_mode == 1) {
+                for (int i = 0; i < nchunks; ++i)
+                  tma_load_2d(a_addr(s) + i * 8192, &tmap_a, full_bar(s), (2 * m_tile + i) * 64, kb * 64);
+              } else {
+                // the k-block's first pixel -> base pixel; every chunk = (filter tap, 64 channels)
+                uint32_t n0i, rem, y0, x0;
+                P.fd_hw.divmod(static_cast<uint32_t>(kb) * 64u, n0i, rem);
+                P.fd_wm.divmod(rem, y0, x0);
+                for (int i = 0; i < nchunks; ++i) {
+                  uint32_t tap, cbk, r, sx;
+                  P.fd_cpb.divmod(static_cast<uint32_t>(2 * m_tile + i), tap, cbk);
+                  P.fd_kw.divmod(tap, r, sx);
+                  tma_load_im2col_4d(a_addr(s) + i * 8192, &tmap_a, full_bar(s), static_cast<int>(cbk) * 64,
+                                     static_cast<int>(x0) * P.i2c_stride + P.i2c_lo,
+                                     static_cast<int>(y0) * P.i2c_stride + P.i2c_lo, static_cast<int>(n0i),
+                                     static_cast<uint16_t>(sx), static_cast<uint16_t>(r));
                 }
-              } else {
-                mbar_arrive_expect_tx(full_bar(s), C::kBBytes);
               }
-              if constexpr (!WGRAD) {
-                const int kcoord = STEM ? kb : P.tap_list[tc] * P.cpb + cb;
-                tma_load_2d(b_addr(s), &tmap_b, full_bar(s), kcoord * BK, n0);
-              } else {
 #pragma unroll
-                for (int i = 0; i < BN / 64; ++i)
-                  tma_load_2d(b_addr(s) + i * 8192, &tmap_b, full_bar(s), n0 + 64 * i, kb * 64);
-              }
+              for (int i = 0; i < BN / 64; ++i)
+                tma_load_2d(b_addr(s) + i * 8192, &tmap_b, full_bar(s), n0 + 64 * i, kb * 64);
             }
           }
-          if constexpr (!WGRAD && !STEM) {
+          if constexpr (!WGRAD) {
             if (++cb == P.cpb) { cb = 0; ++tc; }
           }
           __syncwarp();
         }
       }
     }
-  } else if (warp == kMmaWarp) {
-    // ============================== MMA issuer ==============================
-    if (CTA2 && rank != 0) {
-      // pair peer: no MMAs to issue, nothing to relay (its operand bytes are counted on the leader's barrier)
-    } else {
-      // the whole warp walks the ring (converged: operands stay in uniform registers); one elected lane issues
-      constexpr uint32_t idesc = make_idesc(CTA2 ? 2 * BM : BM, BN, WGRAD ? 1 : 0, WGRAD ? 1 : 0);
-      uint32_t rs = 0, rph = 0, tcount = 0;
-      const uint32_t patch_wp8 = static_cast<uint32_t>(P.patch_wp) * 8u;   // PATCH: one padded row, in 16-byte units
-      for (int t = tile_first; t < tile_end; t += tile_step, ++tcount) {
-        int split, m_tile, n_tile, kb_begin, nk;
-        decode_tile(t, split, m_tile, n_tile, kb_begin, nk);
-        const int acc = tcount & 1;
-        mbar_wait(tempty_bar(acc), ((tcount >> 1) & 1) ^ 1u);     // epilogue(s) have drained this accumulator
-        tcgen05_fence_after();
-        const uint32_t tmem_d = tmem_base + acc * BN;
-        if constexpr (PATCH) {
-          if (tcount == 0) mbar_wait(bres_bar, 0);
-          const int s = static_cast<int>(rs);
-          mbar_wait(full_bar(s), rph);
-          if (++rs == nstages) { rs = 0; rph ^= 1u; }
-          tcgen05_fence_after();
-          if (elect_one()) {
-            // tap tp: the patch displaced by patch_off[tp] rows.  The 128-byte swizzle is a function of the shared-memory
-            // ADDRESS (TMA and UMMA agree on it), so a K-major descriptor may start at any 128-byte row of the patch
-            // with base_offset 0 (tools/exp_shift.cu, profiles/r2_exp_shifted_descriptor.log).  36 MMAs in straight
-            // line: descriptor = stage base + a per-tap constant (rolled, with the offsets read from the parameter
-            // block, the issue loop itself took 2.4x the MMAs' time)
-            // one filter row per iteration of a ROLLED loop (running descriptors, immediates for the column / k offsets):
-            // fully unrolled the compiler kept all 72 descriptors in vector registers and moved them to uniform
-            // registers in front of every MMA
-            uint64_t arow = make_smem_desc(a_addr(s), 16u, 1024u) + (P.transposed ? 2u * patch_wp8 : 0u);
-            uint64_t brow = make_smem_desc(bres_addr, 16u, 1024u);
-            const uint32_t srev = P.transposed ? 16u : 0u;             // dgrad: column displacement 2 - s
-#pragma unroll 1
-            for (int fr = 0; fr < 3; ++fr) {
-#pragma unroll
-              for (int fs = 0; fs < 3; ++fs) {
-                const uint64_t ad = arow + static_cast<uint64_t>(P.transposed ? srev - fs * 8u : fs * 8u);
-#pragma unroll
-                for (int k = 0; k < BK / 16; ++k)
-                  umma_bf16(tmem_d, ad + static_cast<uint64_t>(k * 2),
-                            brow + static_cast<uint64_t>(fs * ((BN * BK * 2) >> 4) + k * 2), idesc,
-                            (fr > 0 || fs > 0 || k > 0) ? 1u : 0u);
-              }
-              arow = P.transposed ? arow - patch_wp8 : arow + patch_wp8;
-              brow += 3u * ((BN * BK * 2) >> 4);
-            }
-            umma_commit(empty_bar(s));
-            umma_commit(tfull_bar(acc));
-          }
-          __syncwarp();
-          continue;
-        }
-        for (int it = 0; it < nk; ++it) {
-          const int s = static_cast<int>(rs);
-          mbar_wait(full_bar(s), rph);
-          if (++rs == nstages) { rs = 0; rph ^= 1u; }
-          tcgen05_fence_after();
-          // K-major: 8-row atoms 1024 B apart; MN-major: 64-wide chunks 8192 B apart (LBO), 8-k atoms 1024 B (SBO)
-          const uint64_t adesc = make_smem_desc(a_addr(s), WGRAD ? 8192u : 16u, 1024u);
-          const uint64_t bdesc =
-              make_smem_desc(b_addr(s), WGRAD ? 8192u : 16u, 1024u);
-          constexpr uint32_t kadv = WGRAD ? (2048u >> 4) : (32u >> 4);   // one UMMA_K (=16) step, in 16-byte units
-          if (elect_one()) {
-#pragma unroll
-            for (int k = 0; k < BK / 16; ++k) {
-              if constexpr (CTA2)
-                umma_bf16_cta2(tmem_d, adesc + static_cast<uint64_t>(k * kadv), bdesc + static_cast<uint64_t>(k * kadv),
-                               idesc, (it > 0 || k > 0) ? 1u : 0u);
-              else
-                umma_bf16(tmem_d, adesc + static_cast<uint64_t>(k * kadv), bdesc + static_cast<uint64_t>(k * kadv), idesc,
-                          (it > 0 || k > 0) ? 1u : 0u);
-            }
-            if constexpr (CTA2) umma_commit_cta2(empty_bar(s));     // frees the stage in both CTAs
-            else umma_commit(empty_bar(s));
-          }
-          __syncwarp();
-        }
-        if (elect_one()) {
-          if constexpr (CTA2) umma_commit_cta2(tfull_bar(acc));     // both CTAs' epilogues may drain their halves
-          else umma_commit(tfull_bar(acc));
-        }
-        __syncwarp();
-      }
-    }
-    __syncwarp();
-  } else {
-    // ============================== epilogue (4 warps; PATCH: two groups of 4) ==============================
-    const int quarter = warp & 3;                 // TMEM lanes [32*quarter, 32*quarter + 32)
-    const int row = quarter * 32 + lane;
-    const int egroup = (PATCH && warp < 4) ? 1 : 0;   // PATCH: group g drains accumulator g (every second tile)
-    const int ewarp = egroup * 4 + quarter;           // index of this warp's staging tile / statistics slots
-    uint32_t tcount = 0;
-    // BN statistics of this warp's rows (fprop with stat_out): running column sums in this warp's smem slots
-    float* stat_sm = reinterpret_cast<float*>(smem_raw + (smem_base - smem_u32(smem_raw)) + C::kStatOffset) +
-                     (WGRAD ? 0 : ewarp * (C::kStatWarpBytes / 4)) + lane;
-    if constexpr (!WGRAD) {
-      if (P.stat_out != nullptr)
-        for (int i = 0; i < (BN / C::kEpiCols) * 4; ++i) stat_sm[i * 32] = 0.f;
-    }
-    // PATCH: tile row m = (yy, xx) in padded coordinates -> pixel offset yy * W + xx inside the tile's image rows (-1: a
-    // dead row); the same for every tile, so decoded once: for this lane's own row and for the 8 rows it stores
-    int patch_rel_own = -1, patch_rel8[8];
-    if constexpr (PATCH) {
-      auto rel = [&](int m) -> int {
-        uint32_t yy, xx;
-        P.fd_wp.divmod(static_cast<uint32_t>(m), yy, xx);
-        return (static_cast<int>(yy) < P.patch_r && static_cast<int>(xx) < P.patch_w) ? static_cast<int>(yy) * P.patch_w + static_cast<int>(xx) : -1;
-      };
-      patch_rel_own = rel(quarter * 32 + lane);
-#pragma unroll
-      for (int i = 0; i < 8; ++i) patch_rel8[i] = rel(quarter * 32 + i * 4 + (lane >> 3));
-    }
-    for (int t = tile_first; t < tile_end; t += tile_step, ++tcount) {
-      int split, m_tile, n_tile, kb_begin, nk;
-      decode_tile(t, split, m_tile, n_tile, kb_begin, nk);
-      const int acc = tcount & 1;
-      if constexpr (PATCH) {
-        if (acc != egroup) continue;               // the other group's tile
-      }
-      int patch_base = 0;                          // PATCH: first output row of the tile's image rows
-      if constexpr (PATCH) {                       // (output rows fit 31 bits: n * h * w < 2^31 is checked on the host)
-        uint32_t img, ty;
-        P.fd_tpi.divmod(static_cast<uint32_t>(t), img, ty);
-        patch_base = static_cast<int>((img * P.patch_h + ty * P.patch_r) * P.patch_w);
-      }
-      int my_orow = 0;                             // PATCH: output row of this lane's own tile row
-      if constexpr (PATCH) my_orow = patch_rel_own >= 0 ? patch_base + patch_rel_own : -1;
-      if constexpr (BSTAT) {
-        // the y rows this warp will need in its statistics passes: pulled into L2 while the tile's MMAs still run
-        long long pr = static_cast<long long>(m_tile) * BM + quarter * 32 + lane;
-        if constexpr (PATCH) pr = my_orow;
-        if (pr >= 0 && pr < P.pixels) {
-          const __nv_bfloat16* yl = P.bst_y + pr * P.ldc + n_tile * BN;
-#pragma unroll
-          for (int j = 0; j < BN / 64; ++j) asm volatile("prefetch.global.L2 [%0];" ::"l"(yl + j * 64));
-        }
-      }
-      mbar_wait(tfull_bar(acc), (tcount >> 1) & 1);
-      tcgen05_fence_after();
-      const uint32_t taddr = tmem_base + acc * BN + (static_cast<uint32_t>(quarter * 32) << 16);
-      const int n0 = n_tile * BN;
-      if constexpr (!WGRAD) {
-        // TMEM -> registers -> bf16 -> this warp's smem staging tile (32 rows x kEpiCols), then the rows go out as
-        // coalesced 16-byte-per-lane stores (one full 128-byte line per row and pass)
-        const uint32_t stage_base = smem_base + C::kEpiOffset + ewarp * C::kEpiWarpBytes;
-        const uint32_t my_row = stage_base + lane * C::kStageRowBytes;
-        constexpr int kLanesPerRow = C::kEpiCols * 2 / 16;      // 8 lanes x 16 B = one 128-byte line
-        constexpr int kRowsPerIter = 32 / kLanesPerRow;         // 4 rows per store iteration
-        constexpr int kIters = 32 / kRowsPerIter;               // 8
-        const int sub = lane / kLanesPerRow, col16 = lane % kLanesPerRow;
-        const long long p0 = static_cast<long long>(m_tile) * BM + quarter * 32;
-        // output row of each of the 8 tile rows this lane stores (-1: out of range), resolved once per tile
-        // (32-bit: the host checks that the output has fewer than 2^31 rows)
-        int orow8[kIters];
-#pragma unroll
-        for (int i = 0; i < kIters; ++i) {
-          const long long p = p0 + i * kRowsPerIter + sub;
-          int orow = (p < P.pixels && nk > 0) ? static_cast<int>(p) : -1;
-          if constexpr (PATCH) orow = patch_rel8[i] >= 0 ? patch_base + patch_rel8[i] : -1;
-          if (orow >= 0 && P.cls_on) {                          // class pixel -> row of the full image
-            const uint32_t pk = pack_pixel(p, P);
-            const int n = (pk >> 18) & 0x1FFF, yy = (pk >> 9) & 0x1FF, xx = pk & 0x1FF;
-            orow = (n * P.full_h + 2 * yy + P.cls_py) * P.full_w + 2 * xx + P.cls_px;
-          }
-          orow8[i] = orow;
-        }
-#pragma unroll 1
-        for (int cb = 0; cb < BN / C::kEpiCols; ++cb) {
-#pragma unroll
-          for (int c = 0; c < C::kEpiCols / 32; ++c) {
-            uint32_t v[32];
-            tmem_ld_32x32(taddr + cb * C::kEpiCols + c * 32, v);
-            tmem_ld_wait();
-            if constexpr (AFFINE) {
-              // per-column scale / shift: the same address in every lane (one broadcast transaction per load)
-              const float4* sc4 = reinterpret_cast<const float4*>(P.epi_scale + n0 + cb * C::kEpiCols + c * 32);
-              const float4* sh4 = reinterpret_cast<const float4*>(P.epi_shift + n0 + cb * C::kEpiCols + c * 32);
-              const bool relu_now = P.epi_relu && P.epi_res == nullptr;    // with a residual the ReLU follows the add
-#pragma unroll
-              for (int q4 = 0; q4 < 8; ++q4) {
-                const float4 a = __ldg(sc4 + q4), b = __ldg(sh4 + q4);
-                float r0 = fmaf(__uint_as_float(v[4 * q4]), a.x, b.x), r1 = fmaf(__uint_as_float(v[4 * q4 + 1]), a.y, b.y);
-                float r2 = fmaf(__uint_as_float(v[4 * q4 + 2]), a.z, b.z), r3 = fmaf(__uint_as_float(v[4 * q4 + 3]), a.w, b.w);
-                if (relu_now) { r0 = fmaxf(r0, 0.f); r1 = fmaxf(r1, 0.f); r2 = fmaxf(r2, 0.f); r3 = fmaxf(r3, 0.f); }
-                v[4 * q4] = __float_as_uint(r0); v[4 * q4 + 1] = __float_as_uint(r1);
-                v[4 * q4 + 2] = __float_as_uint(r2); v[4 * q4 + 3] = __float_as_uint(r3);
-              }
-            }
-#pragma unroll
-            for (int jj = 0; jj < 4; ++jj) {
-              uint32_t pk[4];
-#pragma unroll
-              for (int e = 0; e < 4; ++e) {
-                __nv_bfloat162 h = __floats2bfloat162_rn(__uint_as_float(v[8 * jj + 2 * e]), __uint_as_float(v[8 * jj + 2 * e + 1]));
-                pk[e] = *reinterpret_cast<uint32_t*>(&h);
-                if constexpr (PATCH) {
-                  if (my_orow < 0) pk[e] = 0u;      // dead tile row (padding column / past the tile's image rows): keep it out of the sums
-                }
-              }
-              asm volatile("st.shared.v4.b32 [%0], {%1, %2, %3, %4};" ::"r"(my_row + c * 64 + jj * 16), "r"(pk[0]),
-                           "r"(pk[1]), "r"(pk[2]), "r"(pk[3])
-                           : "memory");
-            }
-          }
-          __syncwarp();
-          // BSTAT: lane l owns columns 2l, 2l+1 of the pass; its 32 y words (one per tile row of this warp; L2 hits
-          // thanks to the prefetch above) are requested now -- the accumulator registers are dead -- and consumed after
-          // the output rows have been stored (requesting them before the TMEM load spilled and measured slower)
-          uint32_t yw[32];
-          if constexpr (BSTAT) {
-            const __nv_bfloat16* yp = P.bst_y + n0 + cb * C::kEpiCols + 2 * lane;
-#pragma unroll
-            for (int r = 0; r < 32; ++r) {
-              if constexpr (PATCH) {
-                const int p = __shfl_sync(0xffffffffu, my_orow, r);
-                yw[r] = p >= 0 ? __ldg(reinterpret_cast<const unsigned int*>(yp + static_cast<long long>(p) * P.ldc)) : 0u;
-              } else {
-                const long long p = p0 + r;
-                yw[r] = p < P.pixels ? __ldg(reinterpret_cast<const unsigned int*>(yp + p * P.ldc)) : 0u;
-              }
-            }
-          }
-          __nv_bfloat16* out_cols = reinterpret_cast<__nv_bfloat16*>(P.out) + n0 + cb * C::kEpiCols + col16 * 8;
-          uint4 resv[kIters];
-          if constexpr (AFFINE) {
-            // residual rows of this pass: all loads issued before the first use
-            if (P.epi_res != nullptr) {
-              const __nv_bfloat16* res_cols = P.epi_res + n0 + cb * C::kEpiCols + col16 * 8;
-#pragma unroll
-              for (int i = 0; i < kIters; ++i)
-                resv[i] = orow8[i] >= 0 ? *reinterpret_cast<const uint4*>(res_cols + static_cast<long long>(orow8[i]) * P.ldc)
-                                        : make_uint4(0, 0, 0, 0);
-            }
-          }
-#pragma unroll
-          for (int i = 0; i < kIters; ++i) {
-            if (orow8[i] >= 0) {
-              uint4 val;
-              asm volatile("ld.shared.v4.b32 {%0, %1, %2, %3}, [%4];"
-                           : "=r"(val.x), "=r"(val.y), "=r"(val.z), "=r"(val.w)
-                           : "r"(stage_base + (i * kRowsPerIter + sub) * C::kStageRowBytes + col16 * 16));
-              if constexpr (AFFINE) {
-                if (P.epi_res != nullptr) {
-                  uint32_t o[4] = {val.x, val.y, val.z, val.w};
-                  const uint32_t rr[4] = {resv[i].x, resv[i].y, resv[i].z, resv[i].w};
-#pragma unroll
-                  for (int e = 0; e < 4; ++e) {
-                    float lo = __uint_as_float(o[e] << 16) + __uint_as_float(rr[e] << 16);
-                    float hi = __uint_as_float(o[e] & 0xffff0000u) + __uint_as_float(rr[e] & 0xffff0000u);
-                    if (P.epi_relu) { lo = fmaxf(lo, 0.f); hi = fmaxf(hi, 0.f); }
-                    __nv_bfloat162 h = __floats2bfloat162_rn(lo, hi);
-                    o[e] = *reinterpret_cast<uint32_t*>(&h);
-                  }
-                  val = make_uint4(o[0], o[1], o[2], o[3]);
-                }
-              }
-              *reinterpret_cast<uint4*>(out_cols + static_cast<long long>(orow8[i]) * P.ldc) = val;
-            }
-          }
-          if constexpr (BSTAT) {
-            // dz = g * [bn(y) > 0] with the forward's own fmaf; S0 += dz, S1 += dz * y (two chains, packed fp32 math)
-            const uint32_t* sp = reinterpret_cast<const uint32_t*>(smem_raw + (stage_base - smem_u32(smem_raw))) + lane;
-            const float2 bsc = __ldg(reinterpret_cast<const float2*>(P.bst_scale + n0 + cb * C::kEpiCols + 2 * lane));
-            const float2 bsh = __ldg(reinterpret_cast<const float2*>(P.bst_shift + n0 + cb * C::kEpiCols + 2 * lane));
-            float2 sa = make_float2(0.f, 0.f), qa = sa, sb = sa, qb = sa;
-#pragma unroll
-            for (int r = 0; r < 32; r += 2) {
-              const uint32_t w0 = sp[r * (C::kStageRowBytes / 4)], w1 = sp[(r + 1) * (C::kStageRowBytes / 4)];
-              float2 g0 = make_float2(__uint_as_float(w0 << 16), __uint_as_float(w0 & 0xffff0000u));
-              float2 g1 = make_float2(__uint_as_float(w1 << 16), __uint_as_float(w1 & 0xffff0000u));
-              const float2 y0 = make_float2(__uint_as_float(yw[r] << 16), __uint_as_float(yw[r] & 0xffff0000u));
-              const float2 y1 = make_float2(__uint_as_float(yw[r + 1] << 16), __uint_as_float(yw[r + 1] & 0xffff0000u));
-              if (!(fmaf(y0.x, bsc.x, bsh.x) > 0.f)) g0.x = 0.f;
-              if (!(fmaf(y0.y, bsc.y, bsh.y) > 0.f)) g0.y = 0.f;
-              if (!(fmaf(y1.x, bsc.x, bsh.x) > 0.f)) g1.x = 0.f;
-              if (!(fmaf(y1.y, bsc.y, bsh.y) > 0.f)) g1.y = 0.f;
-              sa = __fadd2_rn(sa, g0);
-              qa = __ffma2_rn(g0, y0, qa);
-              sb = __fadd2_rn(sb, g1);
-              qb = __ffma2_rn(g1, y1, qb);
-            }
-            float* acc = stat_sm + cb * 4 * 32;
-            acc[0] += sa.x + sb.x;
-            acc[32] += sa.y + sb.y;
-            acc[64] += qa.x + qb.x;
-            acc[96] += qa.y + qb.y;
-          } else if (P.stat_out != nullptr) {
-            // column sums over this warp's 32 rows: lane l owns columns 2l, 2l+1 of the pass (one bf16x2 word per
-            // row; rows past the end of the tensor hold zeros).  Word (36 r + l): conflict-free.  Plain (non-volatile)
-            // loads so that all 32 are in flight together, packed fp32 adds / FMAs (FADD2 / FFMA2), two chains.
-            const uint32_t* sp = reinterpret_cast<const uint32_t*>(smem_raw + (stage_base - smem_u32(smem_raw))) + lane;
-            float2 sa = make_float2(0.f, 0.f), qa = sa, sb = sa, qb = sa;
-#pragma unroll
-            for (int r = 0; r < 32; r += 2) {
-              const uint32_t w0 = sp[r * (C::kStageRowBytes / 4)], w1 = sp[(r + 1) * (C::kStageRowBytes / 4)];
-              const float2 v0 = make_float2(__uint_as_float(w0 << 16), __uint_as_float(w0 & 0xffff0000u));
-              const float2 v1 = make_float2(__uint_as_float(w1 << 16), __uint_as_float(w1 & 0xffff0000u));
-              sa = __fadd2_rn(sa, v0);
-              qa = __ffma2_rn(v0, v0, qa);
-              sb = __fadd2_rn(sb, v1);
-              qb = __ffma2_rn(v1, v1, qb);
-            }
-            float* acc = stat_sm + cb * 4 * 32;
-            acc[0] += sa.x + sb.x;
-            acc[32] += sa.y + sb.y;
-            acc[64] += qa.x + qb.x;
-            acc[96] += qa.y + qb.y;
-          }
-          __syncwarp();                                         // staging tile is reused by the next pass / tile
-        }
-      } else {
-        // partials are stored TRANSPOSED, [split][Cout][K_total]: the 32 lanes of a warp hold 32 consecutive k rows,
-        // so each scalar store below is one coalesced 128-byte line, and the reduce kernel reads/writes along k
-        const int krow = m_tile * BM + row;            // row of the [K_total, Cout] result
-        const int ktot = P.total_chunks * 64;
-        float* out = reinterpret_cast<float*>(P.out) + (static_cast<size_t>(split) * P.ldc + n0) * ktot + krow;
-#pragma unroll 1
-        for (int c = 0; c < BN / 32; ++c) {
-          uint32_t v[32];
-          tmem_ld_32x32(taddr + c * 32, v);
-          tmem_ld_wait();
-          if (krow < ktot) {
-#pragma unroll
-            for (int jj = 0; jj < 32; ++jj)
-              out[static_cast<size_t>(c * 32 + jj) * ktot] = nk > 0 ? __uint_as_float(v[jj]) : 0.f;
-          }
-        }
-      }
-      // accumulator drained: hand it back to the MMA warp
-      tcgen05_fence_before();
-      __syncwarp();
-      if (lane == 0) {
-        if (CTA2 && rank != 0) mbar_arrive_remote(mapa_rank(tempty_bar(acc), 0));   // the leader issues the MMAs
-        else mbar_arrive(tempty_bar(acc));
-      }
-    }
-    if constexpr (!WGRAD) {
-      if (P.stat_out != nullptr) {
-        // one flush per CTA: the four epilogue warps' smem column sums are combined (fixed order -> deterministic)
-        // and written as stat_out[blockIdx.x][0][c] = sums, [1][c] = sums of squares for the BN
-        // columns of this CTA's n_tile.  Every CTA of the launch owns >= 1 tile (grid <= tiles), so every row of
-        // its n_tile's column range is written: the consumer (bn_finalize) reads exactly those, no zero-fill needed.
-        __syncwarp();
-        if constexpr (PATCH) asm volatile("bar.sync 1, 256;" ::: "memory");   // both epilogue groups
-        else asm volatile("bar.sync 1, 128;" ::: "memory");                  // the four epilogue warps
-        const float* all = reinterpret_cast<const float*>(smem_raw + (smem_base - smem_u32(smem_raw)) + C::kStatOffset);
-        constexpr int kWarpFloats = C::kStatWarpBytes / 4;
-        float* dst = P.stat_out + static_cast<size_t>(blockIdx.x) * 2 * P.ldc + fixed_n * BN;
-        if (egroup == 0) {
-          for (int o = quarter * 32 + lane; o < 2 * BN; o += 128) {
-            const int k = o / BN, col = o - k * BN;
-            const int cb = col / C::kEpiCols, ln = (col % C::kEpiCols) >> 1, e = col & 1;
-            const int idx = (cb * 4 + k * 2 + e) * 32 + ln;
-            float v = (all[idx] + all[kWarpFloats + idx]) + (all[2 * kWarpFloats + idx] + all[3 * kWarpFloats + idx]);
-            if constexpr (PATCH)
-              v += (all[4 * kWarpFloats + idx] + all[5 * kWarpFloats + idx]) + (all[6 * kWarpFloats + idx] + all[7 * kWarpFloats + idx]);
-            dst[static_cast<size_t>(k) * P.ldc + col] = v;
-          }
-        }
-      }
-    }
+    return;    // producers are done; the consumers below synchronise among themselves only
   }
 
-  tcgen05_fence_before();
-  __syncwarp();
-  if constexpr (CTA2) cluster_sync_all();   // neither CTA may exit (or free TMEM) while its peer still uses its smem/barriers
-  else __syncthreads();
-  if (warp == kMmaWarp) {
-    tcgen05_fence_after();
-    if constexpr (CTA2) tmem_dealloc_cta2(tmem_base, C::kTmemCols);
-    else tmem_dealloc(tmem_base, C::kTmemCols);
+  // ===== consumers (warpgroups 1, 2) =====
+  const int g = (warp >> 2) - 1;                  // tile rows [64 g, 64 g + 64)
+  const int wq = warp & 3;                        // fragment rows [16 wq, 16 wq + 16) of the warpgroup's 64
+  const int ew = g * 4 + wq;                      // consumer warp 0..7: staging tile / statistics slot
+  const int fr = lane >> 2, fc = 2 * (lane & 3);  // fragment row / first column of this lane
+  float* const stat_sm = reinterpret_cast<float*>(smem_gen + C::kStatOffset) + ew * (2 * BN);
+  if constexpr (!WGRAD) {
+    if (P.stat_out != nullptr)
+      for (int i = lane; i < 2 * BN; i += 32) stat_sm[i] = 0.f;
   }
-}
-
-
-// ---- weight gradient of the 3x3 / stride 1 / pad 1, 64 -> 64 convolutions in the patch-resident form -----------------
-// dW[(r, s, ci), co] = sum over pixels p of X[p + (r - 1, s - 1), ci] * dY[p, co].  The split-K wgrad above re-gathers X
-// once per filter tap (1.44 GB through the L2->SM path at batch 256, tensor pipe 22 % -- profiles/r2_igemm_full.md).
-// Here a k-slab is `patch_r` whole image rows in padded coordinates (row q = (yy, xx) = divmod(q, W + 2)):
-//   * the X patch ((patch_r + 2) x (W + 2) x 64 ch, zero-filled borders) is loaded ONCE and feeds all nine taps: tap
-//     (r, s) is an MN-major descriptor starting r * (W + 2) + s rows into it; two taps form the M = 128 of one MMA, their
-//     64-channel chunks `LBO` = the distance between their start rows apart;
-//   * dY arrives as a (W + 2)-wide box (the two extra columns out of range = zeros) so that its row q matches patch row
-//     q; rows [patch_r * (W + 2), 128) of its slot are zeroed once and never written again;
-//   * all of a CTA's slabs accumulate into the SAME five TMEM accumulators (taps (0,1) (2,3) (4,5) (6,7) (8,-)), which are
-//     written out once at the end as this CTA's split-K partial [Cout][9 * 64] (split index = blockIdx.x).
-// Warps: 0 = TMA, 1 = MMA (+ TMEM owner), 2-5 = final drain (TMEM lane quarter = warp & 3).
-constexpr int kWgpThreads = 192;
-constexpr int kWgpStages = 4, kWgpASlot = 32768, kWgpBSlot = 16384, kWgpStage = kWgpASlot + kWgpBSlot;
-constexpr int kWgpSmemBytes = kWgpStages * kWgpStage + 256 + 1024;
-
-__global__ void __launch_bounds__(kWgpThreads, 1)
-wgrad_patch_kernel(const __grid_constant__ CUtensorMap tmap_x, const __grid_constant__ CUtensorMap tmap_dy,
-                   const IgemmParams P) {
-  extern __shared__ uint8_t smem_raw[];
-  const uint32_t smem_base = (smem_u32(smem_raw) + 1023u) & ~1023u;
-  const uint32_t bar_base = smem_base + kWgpStages * kWgpStage;
-  auto a_addr = [&](int s) { return smem_base + s * kWgpStage; };
-  auto b_addr = [&](int s) { return smem_base + s * kWgpStage + kWgpASlot; };
-  auto full_bar = [&](int s) { return bar_base + 8u * s; };
-  auto empty_bar = [&](int s) { return bar_base + 8u * (kWgpStages + s); };
-  const uint32_t done_bar = bar_base + 8u * (2 * kWgpStages), tmem_holder = bar_base + 8u * (2 * kWgpStages + 1);
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-
-  // the whole ring is zeroed once (generic proxy; made visible to the async proxy before any TMA / MMA touches it): the
-  // TMA boxes cover only the first (patch_r + 2) * wp rows of an X slot and patch_r * wp rows of a dY slot, the MMAs read
-  // 128 K rows of both -- the dY rows past the slab must be zeros, and the X rows they meet must not be stale NaNs
-  for (int i = threadIdx.x; i < kWgpStages * kWgpStage / 16; i += kWgpThreads)
-    asm volatile("st.shared.v4.b32 [%0], {%1, %1, %1, %1};" ::"r"(smem_base + i * 16), "r"(0u) : "memory");
-  fence_proxy_async();
-  if (warp == 1) {
-    if (lane == 0) {
-      for (int s = 0; s < kWgpStages; ++s) {
-        mbar_init(full_bar(s), 1);
-        mbar_init(empty_bar(s), 1);
-      }
-      mbar_init(done_bar, 1);
-      fence_barrier_init();
-    }
-    __syncwarp();
-    tmem_alloc(tmem_holder, 512);
-  }
-  tcgen05_fence_before();
-  __syncthreads();
-  tcgen05_fence_after();
-  uint32_t tmem_base;
-  asm volatile("ld.shared.u32 %0, [%1];" : "=r"(tmem_base) : "r"(tmem_holder));
-
-  const int tile_first = blockIdx.x, tile_step = gridDim.x, tile_end = P.m_tiles;
-  if (warp == 0) {
-    const uint32_t bytes = static_cast<uint32_t>(((P.patch_r + 2) + P.patch_r) * P.patch_wp * 128);
-    uint32_t rs = 0, rph = 0;
-    for (int t = tile_first; t < tile_end; t += tile_step) {
-      uint32_t img, ty;
-      P.fd_tpi.divmod(static_cast<uint32_t>(t), img, ty);
-      const int s = static_cast<int>(rs);
-      mbar_wait(empty_bar(s), rph ^ 1u);
-      if (++rs == kWgpStages) { rs = 0; rph ^= 1u; }
-      if (elect_one()) {
-        const int y0 = static_cast<int>(ty) * P.patch_r;
-        mbar_arrive_expect_tx(full_bar(s), bytes);
-        tma_load_4d(a_addr(s), &tmap_x, full_bar(s), 0, -1, y0 - 1, static_cast<int>(img));
-        tma_load_4d(b_addr(s), &tmap_dy, full_bar(s), 0, 0, y0, static_cast<int>(img));
-      }
-      __syncwarp();
-    }
-  } else if (warp == 1) {
-    constexpr uint32_t idesc = make_idesc(128, 64, 1, 1);
-    const uint32_t wp8 = static_cast<uint32_t>(P.patch_wp) * 8u;      // one padded row in 16-byte units
-    uint32_t rs = 0, rph = 0, first = 1;
-    for (int t = tile_first; t < tile_end; t += tile_step) {
+  // K-major: 8-row atoms 1024 B apart; MN-major: 64-wide chunks 8192 B apart (LBO), 8-k atoms 1024 B (SBO).  This
+  // warpgroup's 64 A rows (wgrad: its 64-channel chunk) start 8192 B into the stage.
+  constexpr uint32_t kLbo = WGRAD ? 8192u : 16u;
+  constexpr uint32_t kadv = WGRAD ? (2048u >> 4) : (32u >> 4);   // one k16 step, in 16-byte units
+  constexpr int kT = WGRAD ? 1 : 0;
+  float acc[BN / 2];
+  uint32_t rs = 0, rph = 0;
+  for (int t = tile_first; t < tile_end; t += tile_step) {
+    int split, m_tile, n_tile, kb_begin, nk;
+    decode_tile(t, split, m_tile, n_tile, kb_begin, nk);
+    int prev = 0;
+    for (int it = 0; it < nk; ++it) {
       const int s = static_cast<int>(rs);
       mbar_wait(full_bar(s), rph);
-      if (++rs == kWgpStages) { rs = 0; rph ^= 1u; }
-      tcgen05_fence_after();
-      if (elect_one()) {
-        // MN-major descriptors: k rows 128 B apart, 8-row atoms 1024 B apart (SBO); the second 64-channel chunk of A
-        // (= the pair's second tap) LBO apart.  Bits [16,30) hold LBO >> 4.
-        const uint64_t abase = make_smem_desc(a_addr(s), 0u, 1024u), bbase = make_smem_desc(b_addr(s), 8192u, 1024u);
-        const uint64_t lbo1 = static_cast<uint64_t>(8u) << 16;                    // next tap = next patch row
-        const uint64_t lbo_wrap = static_cast<uint64_t>(wp8 - 16u) << 16;         // tap (r, 2) -> (r + 1, 0)
-        uint64_t a0 = abase + lbo1, a1 = abase + 16u + lbo_wrap, a2 = abase + (wp8 + 8u) + lbo1,
-                 a3 = abase + 2u * wp8 + lbo1, a4 = abase + (2u * wp8 + 16u) + lbo1, b = bbase;
-#pragma unroll 1
-        for (int ks = 0; ks < 8; ++ks) {                      // 8 x 16 padded positions = the slab's K = 128
-          const uint32_t accum = (first && ks == 0) ? 0u : 1u;
-          umma_bf16(tmem_base + 0 * 64, a0, b, idesc, accum);
-          umma_bf16(tmem_base + 1 * 64, a1, b, idesc, accum);
-          umma_bf16(tmem_base + 2 * 64, a2, b, idesc, accum);
-          umma_bf16(tmem_base + 3 * 64, a3, b, idesc, accum);
-          umma_bf16(tmem_base + 4 * 64, a4, b, idesc, accum);
-          a0 += 128u; a1 += 128u; a2 += 128u; a3 += 128u; a4 += 128u; b += 128u;      // 16 rows x 128 B, in 16-byte units
-        }
-        umma_commit(empty_bar(s));
-      }
-      first = 0;
-      __syncwarp();
-    }
-    if (elect_one()) umma_commit(done_bar);
-    __syncwarp();
-  } else {
-    // final drain: accumulator j holds rows (tap 2j, ci) in lanes 0-63 and (tap 2j + 1, ci) in lanes 64-127
-    const int quarter = warp & 3;
-    const int row = quarter * 32 + lane;
-    mbar_wait(done_bar, 0);
-    tcgen05_fence_after();
-    constexpr int ktot = 9 * 64;
-    float* out = reinterpret_cast<float*>(P.out) + static_cast<size_t>(blockIdx.x) * P.ldc * ktot;
-#pragma unroll 1
-    for (int j = 0; j < 5; ++j) {
-      const int tap = 2 * j + (row >> 6);
-      const int krow = tap * 64 + (row & 63);
-#pragma unroll 1
-      for (int c = 0; c < 2; ++c) {
-        uint32_t v[32];
-        tmem_ld_32x32(tmem_base + j * 64 + c * 32 + (static_cast<uint32_t>(quarter * 32) << 16), v);
-        tmem_ld_wait();
-        if (tap < 9) {
+      if (++rs == nstages) { rs = 0; rph ^= 1u; }
+      if constexpr (!ATMA) fence_proxy_async();   // the gathered rows were written through the generic proxy
+      const uint64_t adesc = make_smem_desc(a_addr(s) + g * 8192, kLbo, 1024u);
+      const uint64_t bdesc = make_smem_desc(b_addr(s), kLbo, 1024u);
+      wgmma_fence_operands(acc);
+      wgmma_fence();
 #pragma unroll
-          for (int jj = 0; jj < 32; ++jj) out[static_cast<size_t>(c * 32 + jj) * ktot + krow] = __uint_as_float(v[jj]);
+      for (int k = 0; k < BK / 16; ++k)
+        wgmma_bf16<BN, kT, kT>(acc, adesc + static_cast<uint64_t>(k * kadv), bdesc + static_cast<uint64_t>(k * kadv),
+                               (it > 0 || k > 0) ? 1u : 0u);
+      wgmma_commit();
+      wgmma_fence_operands(acc);
+      // one k-block stays in flight: once the previous one has completed, its stage goes back to the producer
+      if (it > 0) {
+        wgmma_wait<1>();
+        if (lane == 0) mbar_arrive(empty_bar(prev));
+      }
+      prev = s;
+    }
+    wgmma_wait<0>();
+    wgmma_fence_operands(acc);
+    if (nk > 0 && lane == 0) mbar_arrive(empty_bar(prev));
+    const int n0 = n_tile * BN;
+
+    if constexpr (!WGRAD) {
+      // registers -> bf16 staging tile -> coalesced row stores; BN statistics / moments sum the staged (stored) values
+      const uint32_t stage_base = smem_base + C::kEpiOffset + ew * C::kEpiWarpBytes;
+      const bool relu_now = AFFINE && P.epi_relu && P.epi_res == nullptr;    // with a residual the ReLU follows the add
+#pragma unroll
+      for (int j = 0; j < BN / 8; ++j) {
+        const int col = 8 * j + fc;
+        float v0 = acc[4 * j], v1 = acc[4 * j + 1], v2 = acc[4 * j + 2], v3 = acc[4 * j + 3];
+        if constexpr (AFFINE) {
+          const float2 a = __ldg(reinterpret_cast<const float2*>(P.epi_scale + n0 + col));
+          const float2 b = __ldg(reinterpret_cast<const float2*>(P.epi_shift + n0 + col));
+          v0 = fmaf(v0, a.x, b.x); v1 = fmaf(v1, a.y, b.y); v2 = fmaf(v2, a.x, b.x); v3 = fmaf(v3, a.y, b.y);
+          if (relu_now) { v0 = fmaxf(v0, 0.f); v1 = fmaxf(v1, 0.f); v2 = fmaxf(v2, 0.f); v3 = fmaxf(v3, 0.f); }
+        }
+        __nv_bfloat162 h0 = __floats2bfloat162_rn(v0, v1), h1 = __floats2bfloat162_rn(v2, v3);
+        asm volatile("st.shared.b32 [%0], %1;" ::"r"(stage_base + fr * C::kStageRowBytes + col * 2),
+                     "r"(*reinterpret_cast<uint32_t*>(&h0)) : "memory");
+        asm volatile("st.shared.b32 [%0], %1;" ::"r"(stage_base + (fr + 8) * C::kStageRowBytes + col * 2),
+                     "r"(*reinterpret_cast<uint32_t*>(&h1)) : "memory");
+      }
+      __syncwarp();
+      constexpr int kLanesPerRow = BN * 2 / 16;           // 16-byte pieces of one output row
+      constexpr int kRowsPerIter = 32 / kLanesPerRow;
+      constexpr int kIters = 16 / kRowsPerIter;
+      const int sub = lane / kLanesPerRow, col16 = lane % kLanesPerRow;
+      const long long p0 = static_cast<long long>(m_tile) * BM + g * 64 + wq * 16;
+      __nv_bfloat16* out_cols = reinterpret_cast<__nv_bfloat16*>(P.out) + n0 + col16 * 8;
+#pragma unroll
+      for (int i = 0; i < kIters; ++i) {
+        const int rl = i * kRowsPerIter + sub;
+        const long long p = p0 + rl;
+        // output row (32-bit: the host checks that the output has fewer than 2^31 rows)
+        int orow = (p < P.pixels && nk > 0) ? static_cast<int>(p) : -1;
+        if (orow >= 0 && P.cls_on) {                          // class pixel -> row of the full image
+          const uint32_t pk = pack_pixel(p, P);
+          const int n = (pk >> 18) & 0x1FFF, yy = (pk >> 9) & 0x1FF, xx = pk & 0x1FF;
+          orow = (n * P.full_h + 2 * yy + P.cls_py) * P.full_w + 2 * xx + P.cls_px;
+        }
+        if (orow >= 0) {
+          uint4 val;
+          asm volatile("ld.shared.v4.b32 {%0, %1, %2, %3}, [%4];"
+                       : "=r"(val.x), "=r"(val.y), "=r"(val.z), "=r"(val.w)
+                       : "r"(stage_base + rl * C::kStageRowBytes + col16 * 16));
+          if constexpr (AFFINE) {
+            if (P.epi_res != nullptr) {
+              const uint4 rv = *reinterpret_cast<const uint4*>(P.epi_res + n0 + col16 * 8 + static_cast<long long>(orow) * P.ldc);
+              uint32_t o[4] = {val.x, val.y, val.z, val.w};
+              const uint32_t rr[4] = {rv.x, rv.y, rv.z, rv.w};
+#pragma unroll
+              for (int e = 0; e < 4; ++e) {
+                float lo = __uint_as_float(o[e] << 16) + __uint_as_float(rr[e] << 16);
+                float hi = __uint_as_float(o[e] & 0xffff0000u) + __uint_as_float(rr[e] & 0xffff0000u);
+                if (P.epi_relu) { lo = fmaxf(lo, 0.f); hi = fmaxf(hi, 0.f); }
+                __nv_bfloat162 h = __floats2bfloat162_rn(lo, hi);
+                o[e] = *reinterpret_cast<uint32_t*>(&h);
+              }
+              val = make_uint4(o[0], o[1], o[2], o[3]);
+            }
+          }
+          *reinterpret_cast<uint4*>(out_cols + static_cast<long long>(orow) * P.ldc) = val;
+        }
+      }
+      if (BSTAT || P.stat_out != nullptr) {
+        // lane l owns the column pairs l (and l + 32 at BN = 128) of the tile: one bf16x2 word per staged row (rows
+        // past the end of the tensor hold zeros: their A rows were zero-filled)
+#pragma unroll
+        for (int h = 0; h < BN / 64; ++h) {
+          const int col = 2 * (lane + 32 * h);
+          float s0 = 0.f, s1 = 0.f, q0 = 0.f, q1 = 0.f;
+          float2 bsc = make_float2(0.f, 0.f), bsh = bsc;
+          if constexpr (BSTAT) {
+            bsc = __ldg(reinterpret_cast<const float2*>(P.bst_scale + n0 + col));
+            bsh = __ldg(reinterpret_cast<const float2*>(P.bst_shift + n0 + col));
+          }
+#pragma unroll
+          for (int r = 0; r < 16; ++r) {
+            uint32_t w;
+            asm volatile("ld.shared.b32 %0, [%1];" : "=r"(w) : "r"(stage_base + r * C::kStageRowBytes + col * 2));
+            float g0 = __uint_as_float(w << 16), g1 = __uint_as_float(w & 0xffff0000u);
+            if constexpr (BSTAT) {
+              // dz = g * [bn(y) > 0] with the forward's own fmaf; S0 += dz, S1 += dz * y
+              const long long p = p0 + r;
+              const uint32_t yw = p < P.pixels ? __ldg(reinterpret_cast<const unsigned int*>(P.bst_y + p * P.ldc + n0 + col)) : 0u;
+              const float y0 = __uint_as_float(yw << 16), y1 = __uint_as_float(yw & 0xffff0000u);
+              if (!(fmaf(y0, bsc.x, bsh.x) > 0.f)) g0 = 0.f;
+              if (!(fmaf(y1, bsc.y, bsh.y) > 0.f)) g1 = 0.f;
+              s0 += g0; s1 += g1;
+              q0 = fmaf(g0, y0, q0); q1 = fmaf(g1, y1, q1);
+            } else {
+              s0 += g0; s1 += g1;
+              q0 = fmaf(g0, g0, q0); q1 = fmaf(g1, g1, q1);
+            }
+          }
+          stat_sm[col] += s0;
+          stat_sm[col + 1] += s1;
+          stat_sm[BN + col] += q0;
+          stat_sm[BN + col + 1] += q1;
+        }
+      }
+      __syncwarp();                                         // staging tile is reused by the next tile
+    } else {
+      // partials are stored TRANSPOSED, [split][Cout][K_total] (the reduce kernel walks k)
+      const int ktot = P.total_chunks * 64;
+      const int krow = m_tile * BM + g * 64 + wq * 16 + fr;   // row of the [K_total, Cout] result
+      float* out = reinterpret_cast<float*>(P.out) + (static_cast<size_t>(split) * P.ldc + n0) * ktot;
+#pragma unroll
+      for (int j = 0; j < BN / 8; ++j) {
+        const size_t c0 = static_cast<size_t>(8 * j + fc) * ktot;
+#pragma unroll
+        for (int e = 0; e < 2; ++e) {
+          if (krow < ktot) out[c0 + e * ktot + krow] = nk > 0 ? acc[4 * j + e] : 0.f;
+          if (krow + 8 < ktot) out[c0 + e * ktot + krow + 8] = nk > 0 ? acc[4 * j + 2 + e] : 0.f;
         }
       }
     }
   }
-  tcgen05_fence_before();
-  __syncthreads();
-  if (warp == 1) {
-    tcgen05_fence_after();
-    tmem_dealloc(tmem_base, 512);
+  if constexpr (!WGRAD) {
+    if (P.stat_out != nullptr) {
+      // one flush per CTA: the eight consumer warps' smem column sums are combined (fixed order -> deterministic) and
+      // written as stat_out[blockIdx.x][0][c] = sums, [1][c] = sums of squares for the BN columns of this CTA's
+      // n_tile.  Every CTA of the launch owns >= 1 tile (grid <= tiles), so every row of its n_tile's column range
+      // is written: the consumer (bn_finalize) reads exactly those, no zero-fill needed.
+      asm volatile("bar.sync 1, 256;" ::: "memory");       // the two consumer warpgroups
+      const float* all = reinterpret_cast<const float*>(smem_gen + C::kStatOffset);
+      float* dst = P.stat_out + static_cast<size_t>(blockIdx.x) * 2 * P.ldc + fixed_n * BN;
+      for (int o = static_cast<int>(threadIdx.x) - kProducerThreads; o < 2 * BN; o += kThreads - kProducerThreads) {
+        const int k = o / BN, col = o - k * BN;
+        const float v = ((all[o] + all[2 * BN + o]) + (all[4 * BN + o] + all[6 * BN + o])) +
+                        ((all[8 * BN + o] + all[10 * BN + o]) + (all[12 * BN + o] + all[14 * BN + o]));
+        dst[static_cast<size_t>(k) * P.ldc + col] = v;
+      }
+    }
   }
 }
 
@@ -1155,7 +721,6 @@ int make_tmap_im2col_bf16(CUtensorMap* tm, const void* ptr, int c, int w, int h,
     reinterpret_cast<uint64_t*>(tm)[1] &= ~(1ull << 21);
   return DIRB200_OK;
 }
-
 static thread_local StatLayout t_last_layout{};     // row layout of the statistics the most recent fprop launch wrote
 
 // Host-side completion of the launch parameters: reciprocal constants for every run-time divisor the kernel meets and
@@ -1168,8 +733,6 @@ static IgemmParams finish_params(const IgemmParams& P) {
   Q.fd_kw = make_fastdiv(static_cast<uint32_t>(Q.kw > 0 ? Q.kw : 1));
   Q.fd_ntiles = make_fastdiv(static_cast<uint32_t>(Q.n_tiles > 0 ? Q.n_tiles : 1));
   Q.fd_persplit = make_fastdiv(static_cast<uint32_t>(Q.m_tiles * Q.n_tiles > 0 ? Q.m_tiles * Q.n_tiles : 1));
-  Q.fd_tpi = make_fastdiv(static_cast<uint32_t>(Q.patch_r > 0 ? Q.patch_h / Q.patch_r : 1));
-  Q.fd_wp = make_fastdiv(static_cast<uint32_t>(Q.patch_wp > 0 ? Q.patch_wp : 1));
   const int nt = Q.ntaps_c < kMaxTaps ? Q.ntaps_c : kMaxTaps;
   for (int i = 0; i < kMaxTaps; ++i) {
     Q.tap_eoff[i] = 0;
@@ -1199,79 +762,24 @@ static IgemmParams finish_params(const IgemmParams& P) {
   return Q;
 }
 
-template <int BN, bool WGRAD, bool STEM, bool ATMA = false, bool AFFINE = false, bool BSTAT = false, bool PATCH = false>
+template <int BN, bool WGRAD, bool STEM, bool ATMA = false, bool AFFINE = false, bool BSTAT = false>
 static int launch_igemm_impl(const CUtensorMap& tm, const CUtensorMap& tma, const IgemmParams& Qin, cudaStream_t st) {
-  using C = Cfg<BN, !WGRAD, false, PATCH>;
+  using C = Cfg<BN, !WGRAD>;
   const IgemmParams Q = finish_params(Qin);
   static bool configured = false;
   if (!configured) {
-    DIRB_CUDA(cudaFuncSetAttribute(igemm_kernel<BN, WGRAD, STEM, false, ATMA, AFFINE, BSTAT, PATCH>,
+    DIRB_CUDA(cudaFuncSetAttribute(igemm_kernel<BN, WGRAD, STEM, ATMA, AFFINE, BSTAT>,
                                    cudaFuncAttributeMaxDynamicSharedMemorySize, C::kSmemBytes));
     configured = true;
   }
   const int grid = Q.num_tiles < num_sms() ? Q.num_tiles : num_sms();
   t_last_layout = StatLayout{grid, Q.n_tiles, BN, 1};
-  igemm_kernel<BN, WGRAD, STEM, false, ATMA, AFFINE, BSTAT, PATCH><<<grid, (ATMA && !PATCH) ? kThreads - kProducerThreads : kThreads, C::kSmemBytes, st>>>(tm, tma, Q);
+  igemm_kernel<BN, WGRAD, STEM, ATMA, AFFINE, BSTAT><<<grid, kThreads, C::kSmemBytes, st>>>(tm, tma, Q);
   DIRB_LAUNCHED();
   return DIRB200_OK;
 }
 
-// CTA-pair variant: (2,1,1) clusters, one pair per two SMs; Q.m_tiles / Q.num_tiles count 256-row pair tiles.
-template <int BN, bool AFFINE = false, bool BSTAT = false>
-static int launch_igemm_cta2(const CUtensorMap& tm, const CUtensorMap& tma, const IgemmParams& Qin, cudaStream_t st) {
-  using C = Cfg<BN, true, true>;
-  const IgemmParams Q = finish_params(Qin);
-  auto kern = igemm_kernel<BN, false, false, true, true, AFFINE, BSTAT>;
-  static bool configured = false;
-  if (!configured) {
-    DIRB_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, C::kSmemBytes));
-    configured = true;
-  }
-  cudaLaunchConfig_t cfg{};
-  cfg.gridDim = dim3(num_sms() & ~1, 1, 1);
-  cfg.blockDim = dim3(kThreads - kProducerThreads, 1, 1);     // TMA-fed: no gather warps
-  cfg.dynamicSmemBytes = C::kSmemBytes;
-  cfg.stream = st;
-  cudaLaunchAttribute attr[1];
-  attr[0].id = cudaLaunchAttributeClusterDimension;
-  attr[0].val.clusterDim.x = 2;
-  attr[0].val.clusterDim.y = 1;
-  attr[0].val.clusterDim.z = 1;
-  cfg.attrs = attr;
-  cfg.numAttrs = 1;
-  // the persistent tile walk assumes every cluster of the grid is resident at once: cap the grid at the number of
-  // CTA pairs the device can actually co-schedule (a TPC with one SM fused off cannot host a pair)
-  static int max_pairs = 0;
-  if (max_pairs == 0) {
-    int mc = 0;
-    if (cudaOccupancyMaxActiveClusters(&mc, kern, &cfg) != cudaSuccess || mc <= 0) {
-      (void)cudaGetLastError();
-      mc = num_sms() / 2;
-    }
-    max_pairs = mc < num_sms() / 2 ? mc : num_sms() / 2;
-    if (getenv("DIRB200_VERBOSE")) fprintf(stderr, "dirb200: igemm CTA pairs BN=%d: %d co-resident clusters\n", BN, max_pairs);
-  }
-  const int pairs = Q.num_tiles < max_pairs ? Q.num_tiles : max_pairs;
-  cfg.gridDim = dim3(2 * pairs, 1, 1);
-  t_last_layout = StatLayout{2 * pairs, Q.n_tiles, BN, 2};
-  DIRB_CUDA(cudaLaunchKernelEx(&cfg, kern, tm, tma, Q));
-  DIRB_LAUNCHED();
-  return DIRB200_OK;
-}
-
-// CTA pairs (tcgen05 cta_group::2, 256 x 256 pair tiles, both operands by TMA) carry the fprop / stride-1 dgrad GEMMs
-// whose tile is 256 wide and at least 4 k-blocks deep: each CTA then stages 32 KB instead of 48 KB per k-block, and
-// those layers run at the L2->SM delivery limit (measured, profiles/r2_conv_layers.md: 5-15 % faster; shallower or
-// narrower GEMMs are epilogue / DRAM bound and lose a little to the cluster handshakes).  DIRB200_CTA2=0 disables.
-static bool pairs_enabled() {
-  static const bool on = [] {
-    const char* e = getenv("DIRB200_CTA2");
-    return !(e != nullptr && e[0] == '0');
-  }();
-  return on;
-}
-
-// tma != nullptr: the A operand is a plain [pixels][channels] matrix (1x1 stride-1 conv) and is loaded by TMA too
+// tma != nullptr: the A operand is loaded by TMA too (tiled or im2col map, P.a_mode)
 template <int BN, bool WGRAD, bool STEM>
 static int launch_igemm(const CUtensorMap& tm, const IgemmParams& P, int m_tiles, int splits, cudaStream_t st,
                         const CUtensorMap* tma = nullptr) {
@@ -1294,23 +802,12 @@ static int launch_igemm(const CUtensorMap& tm, const IgemmParams& P, int m_tiles
   return launch_igemm_impl<BN, WGRAD, STEM>(tm, tm, Q, st);
 }
 
-// GEMM-N tile width: 256 halves the A-operand traffic per FLOP (the conv kernels are bound by L2->SM operand
-// bandwidth), used when it still leaves >= 2 tiles per SM; else 128; 64 for 64-channel layers.
-// gather_fed (A operand through the cp.async gather, i.e. every conv that is not a plain 1x1 GEMM): measured, the
-// gather sustains one 16 KB A tile per ~0.6 us per SM whatever BN is, so the launch time is (waves x k-blocks) and the
-// widest tile always wins once at least half of the SMs have work.
-static int pick_bn(int n_dim, long long m_tiles, bool gather_fed = false) {
-  if (n_dim % 256 == 0) {
-    const long long t256 = m_tiles * (n_dim / 256);
-    if (t256 >= 2LL * num_sms() || (gather_fed && 2 * t256 >= num_sms())) return 256;
-  }
-  if (n_dim % 128 == 0) return 128;
-  return 64;
-}
+// GEMM-N tile width: 128 where N allows (a consumer warpgroup's 64 x 128 fp32 accumulators take 64 registers per
+// thread; a 256-wide tile would need 128 and leave too few for the epilogue at three warpgroups per SM), else 64.
+static int pick_bn(int n_dim) { return n_dim % 128 == 0 ? 128 : 64; }
 
-#define DISPATCH_BN(bn, WG, ST, ...)                                        \
-  ((bn) == 256 ? launch_igemm<256, WG, ST>(__VA_ARGS__)                     \
-               : ((bn) == 128 ? launch_igemm<128, WG, ST>(__VA_ARGS__) : launch_igemm<64, WG, ST>(__VA_ARGS__)))
+#define DISPATCH_BN(bn, WG, ST, ...) \
+  ((bn) == 128 ? launch_igemm<128, WG, ST>(__VA_ARGS__) : launch_igemm<64, WG, ST>(__VA_ARGS__))
 
 static int check_shape(const ConvShape& s, bool stem, const char* who) {
   DIRB_CHECK_ARG(s.n > 0 && s.h > 0 && s.w > 0 && s.kh > 0 && s.kw > 0 && s.stride > 0 && s.pad >= 0,
@@ -1348,85 +845,6 @@ static bool im2col_enabled() {
   return on && atma_enabled();
 }
 
-// CTA-pair launch of an fprop / dgrad GEMM: B = wmat [n_dim][ktot] (K-major), each CTA TMA-loads bn/2 of its rows.
-static int launch_cta2(const __nv_bfloat16* wmat, int ktot, int n_dim, const IgemmParams& P, int m_tiles,
-                       cudaStream_t st, const CUtensorMap& tma) {
-  CUtensorMap tm;
-  if (int rc = make_tmap_bf16_2d(&tm, wmat, ktot, n_dim, static_cast<uint64_t>(ktot) * 2, 128)) return rc;
-  IgemmParams Q = P;
-  Q.m_tiles = (m_tiles + 1) / 2;                 // 256-row pair tiles
-  Q.num_tiles = Q.m_tiles * P.n_tiles;
-  if (Q.epi_scale != nullptr) return launch_igemm_cta2<256, true>(tm, tma, Q, st);
-  if (Q.bst_y != nullptr) return launch_igemm_cta2<256, false, true>(tm, tma, Q, st);
-  return launch_igemm_cta2<256>(tm, tma, Q, st);
-}
-static bool want_pairs(int bn, int num_kblocks) { return pairs_enabled() && bn == 256 && num_kblocks >= 4; }
-
-// Patch-resident form for the 3x3 / stride 1 / pad 1, 64 -> 64 convolutions (layer1's conv2: fprop and dgrad).  With a
-// 128 x 64 tile the im2col form pulls every input pixel nine times plus the weight tile per k-block through the L2->SM
-// path (1.39 GB per launch at batch 256, 11.3 TB/s = the delivery limit, tensor pipe 25 % -- profiles/r2_igemm_full.md);
-// here a tile is `r` whole image rows in padded coordinates, its input patch is loaded ONCE by a tiled TMA box
-// (zero-filled borders) and the nine taps are UMMA descriptors displaced inside that patch; the weights stay resident.
-// DIRB200_PATCH=0 disables.
-static bool patch_enabled() {
-  static const bool on = [] {
-    const char* e = getenv("DIRB200_PATCH");
-    return !(e != nullptr && e[0] == '0');
-  }();
-  return on && im2col_enabled();
-}
-// rows per tile: the largest divisor r of h with r * (w + 2) <= 128 (0: shape not supported)
-static int patch_rows(int h, int w, int channels, int kh, int kw, int stride, int pad, int n_dim) {
-  if (!patch_enabled() || kh != 3 || kw != 3 || stride != 1 || pad != 1 || channels != 64 || n_dim != 64) return 0;
-  const int wp = w + 2;
-  if (wp > 128 || (2 * wp + 2 + 128) * 128 > 32768) return 0;
-  for (int r = 128 / wp; r >= 1; --r)
-    if (h % r == 0 && r + 2 <= 256) return r;
-  return 0;
-}
-// tiled 4-D map of an NHWC bf16 tensor with 64 channels: boxes of (w + 2) columns x `box_rows` rows x 64 channels
-// (coordinates may start at -1: the out-of-range border arrives as zeros)
-static int make_tmap_patch(CUtensorMap* tm, const __nv_bfloat16* src, int n, int h, int w, int box_rows) {
-  typedef CUresult (*Fn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*, const cuuint64_t*,
-                         const cuuint32_t*, const cuuint32_t*, CUtensorMapInterleave, CUtensorMapSwizzle,
-                         CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
-  Fn fn = reinterpret_cast<Fn>(encode_fn());
-  if (!fn) {
-    set_error("cuTensorMapEncodeTiled entry point not available");
-    return DIRB200_ERR_CUDA;
-  }
-  cuuint64_t dims[4] = {64, (cuuint64_t)w, (cuuint64_t)h, (cuuint64_t)n};
-  cuuint64_t strides[3] = {128, (cuuint64_t)w * 128, (cuuint64_t)h * w * 128};
-  cuuint32_t box[4] = {64, (cuuint32_t)(w + 2), (cuuint32_t)box_rows, 1};
-  cuuint32_t estr[4] = {1, 1, 1, 1};
-  CUresult cr = fn(tm, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 4, const_cast<__nv_bfloat16*>(src), dims, strides, box, estr,
-                   CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
-                   CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-  if (cr != CUDA_SUCCESS) {
-    set_error("cuTensorMapEncodeTiled (patch) failed (%d) w=%d h=%d n=%d rows=%d", (int)cr, w, h, n, box_rows);
-    return DIRB200_ERR_CUDA;
-  }
-  return DIRB200_OK;
-}
-
-// src: the tensor the taps slide over ([n, h, w, 64]); wmat: [64][9 * 64] K-major; flipped: dgrad (tap (r, s) reads the
-// patch displaced by (2 - r, 2 - s))
-static int launch_patch(const __nv_bfloat16* src, const __nv_bfloat16* wmat, IgemmParams P, int n, int h, int w, int r,
-                        bool flipped, cudaStream_t st) {
-  CUtensorMap ta, tb;
-  if (int rc = make_tmap_patch(&ta, src, n, h, w, r + 2)) return rc;
-  if (int rc = make_tmap_bf16_2d(&tb, wmat, 9 * 64, 64, 9 * 64 * 2, 64)) return rc;
-  P.patch_r = r; P.patch_wp = w + 2; P.patch_h = h; P.patch_w = w;
-  P.transposed = flipped ? 1 : 0;
-  P.a_mode = 3;
-  P.n_tiles = 1;
-  P.m_tiles = n * (h / r);
-  P.num_tiles = P.m_tiles;
-  P.num_kblocks = 9;
-  if (P.bst_y != nullptr) return launch_igemm_impl<64, false, false, true, false, true, true>(tb, ta, P, st);
-  return launch_igemm_impl<64, false, false, true, false, false, true>(tb, ta, P, st);
-}
-
 // Y[n,ho,wo,cout] = conv(X[n,h,w,cin], W[cout][kh][kw][cin])
 static int conv_fprop_impl(const __nv_bfloat16* x, const __nv_bfloat16* w, __nv_bfloat16* y, const ConvShape& s, bool stem,
                            cudaStream_t st, float* stat_partial, const ConvEpilogue* epi);
@@ -1462,12 +880,8 @@ static int conv_fprop_impl(const __nv_bfloat16* x, const __nv_bfloat16* w, __nv_
   if (epi) {
     P.epi_scale = epi->scale; P.epi_shift = epi->shift; P.epi_res = epi->residual; P.epi_relu = epi->relu ? 1 : 0;
   }
-  if (!stem && !epi) {
-    if (const int pr = patch_rows(s.h, s.w, s.cin, s.kh, s.kw, s.stride, s.pad, s.cout))
-      return launch_patch(x, w, P, s.n, s.h, s.w, pr, false, st);
-  }
   const int m_tiles = static_cast<int>((P.pixels + BM - 1) / BM);
-  const int bn = pick_bn(s.cout, m_tiles, !is_plain_gemm(s, stem));
+  const int bn = pick_bn(s.cout);
   P.n_tiles = s.cout / bn;
   CUtensorMap tm, ta;
   bool tma_fed = false;
@@ -1483,7 +897,6 @@ static int conv_fprop_impl(const __nv_bfloat16* x, const __nv_bfloat16* w, __nv_
     P.a_mode = 2; P.i2c_stride = s.stride; P.i2c_lo = -s.pad;
     tma_fed = true;
   }
-  if (tma_fed && want_pairs(bn, P.num_kblocks)) return launch_cta2(w, ktot, s.cout, P, m_tiles, st, ta);
   if (int rc = make_tmap_bf16_2d(&tm, w, ktot, s.cout, static_cast<uint64_t>(ktot) * 2, bn)) return rc;
   if (stem) return DISPATCH_BN(bn, false, true, tm, P, m_tiles, 1, st);
   if (tma_fed) return DISPATCH_BN(bn, false, false, tm, P, m_tiles, 1, st, &ta);
@@ -1512,19 +925,15 @@ int conv_dgrad(const __nv_bfloat16* dy, const __nv_bfloat16* wt, __nv_bfloat16* 
   if (bnm) {
     P.bst_y = bnm->y; P.bst_scale = bnm->scale; P.bst_shift = bnm->shift; P.stat_out = bnm->partial;
   }
+  const int bn = pick_bn(s.cin);
   CUtensorMap tm;
+  if (int rc = make_tmap_bf16_2d(&tm, wt, ktot, s.cin, static_cast<uint64_t>(ktot) * 2, bn)) return rc;
   if (s.stride == 1) {
     P.pixels = static_cast<long long>(s.n) * s.h * s.w;
     P.ntaps_c = s.kh * s.kw;
     for (int i = 0; i < kMaxTaps; ++i) P.tap_list[i] = i;
     P.num_kblocks = ktot / 64;
-    if (const int pr = patch_rows(s.ho, s.wo, s.cout, s.kh, s.kw, s.stride, s.pad, s.cin)) {
-      const int rc = launch_patch(dy, wt, P, s.n, s.ho, s.wo, pr, true, st);
-      if (bnm && bnm->layout) *bnm->layout = t_last_layout;
-      return rc;
-    }
     const int m_tiles = static_cast<int>((P.pixels + BM - 1) / BM);
-    const int bn = pick_bn(s.cin, m_tiles, !is_plain_gemm(s, false));
     P.n_tiles = s.cin / bn;
     CUtensorMap ta;
     bool tma_fed = false;
@@ -1541,14 +950,8 @@ int conv_dgrad(const __nv_bfloat16* dy, const __nv_bfloat16* wt, __nv_bfloat16* 
       P.a_mode = 2; P.i2c_stride = 1; P.i2c_lo = lo;
       tma_fed = true;
     }
-    int rc;
-    if (tma_fed && want_pairs(bn, P.num_kblocks)) {
-      rc = launch_cta2(wt, ktot, s.cin, P, m_tiles, st, ta);
-    } else {
-      if ((rc = make_tmap_bf16_2d(&tm, wt, ktot, s.cin, static_cast<uint64_t>(ktot) * 2, bn))) return rc;
-      rc = tma_fed ? DISPATCH_BN(bn, false, false, tm, P, m_tiles, 1, st, &ta)
-                   : DISPATCH_BN(bn, false, false, tm, P, m_tiles, 1, st);
-    }
+    const int rc = tma_fed ? DISPATCH_BN(bn, false, false, tm, P, m_tiles, 1, st, &ta)
+                           : DISPATCH_BN(bn, false, false, tm, P, m_tiles, 1, st);
     if (bnm && bnm->layout) *bnm->layout = t_last_layout;
     return rc;
   }
@@ -1577,9 +980,7 @@ int conv_dgrad(const __nv_bfloat16* dy, const __nv_bfloat16* wt, __nv_bfloat16* 
     Q.pixels = static_cast<long long>(s.n) * Q.hm * Q.wm;
     Q.num_kblocks = Q.ntaps_c * Q.cpb;
     const int m_tiles = static_cast<int>((Q.pixels + BM - 1) / BM);
-    const int bn = pick_bn(s.cin, m_tiles, true);
     Q.n_tiles = s.cin / bn;
-    if (int rc = make_tmap_bf16_2d(&tm, wt, ktot, s.cin, static_cast<uint64_t>(ktot) * 2, bn)) return rc;
     if (im2col_enabled()) {
       // the class is a stride-1 "convolution" over the dy grid whose taps sit at offsets (py + pad - r) / 2: im2col-mode
       // TMA with the base-pixel box [lo, lo + class grid) (out-of-range dy pixels arrive as zeros)
@@ -1602,17 +1003,12 @@ int conv_dgrad(const __nv_bfloat16* dy, const __nv_bfloat16* wt, __nv_bfloat16* 
   return DIRB200_OK;
 }
 
-static int wgrad_bn(const ConvShape& s) { return s.cout % 256 == 0 ? 256 : (s.cout % 128 == 0 ? 128 : 64); }
+static int wgrad_bn(const ConvShape& s) { return pick_bn(s.cout); }
 
 // Split-K factor of the wgrad GEMM (K = pixels).  The persistent CTAs walk tiles x splits work items in waves of
-// num_sms; one item costs its k-blocks plus an epilogue worth ~6 k-blocks (128 x BN fp32 partials), so the launch
-// costs about waves x (k-blocks per split + 6).  Picking the minimiser avoids the "one item too many" third wave the
-// old ceil(2 * sms / tiles) rule produced for the 3x3 layers (e.g. 9 tiles x 33 splits = 297 items on 148 SMs).
+// num_sms; one item costs its k-blocks plus an epilogue worth ~6 k-blocks (128 x BN fp32 partials; an estimate, not
+// re-measured on H100), so a launch costs about waves x (k-blocks per split + 6); the minimiser avoids straggler waves.
 int conv_wgrad_splits(const ConvShape& s) {
-  if (const int pr = patch_rows(s.h, s.w, s.cin, s.kh, s.kw, s.stride, s.pad, s.cout)) {
-    const int slabs = s.n * (s.h / pr);             // patch form: one partial per CTA
-    return slabs < num_sms() ? slabs : num_sms();
-  }
   const long long pixels = static_cast<long long>(s.n) * s.ho * s.wo;
   const int kblocks = static_cast<int>((pixels + 63) / 64);
   const int chunks = s.kh * s.kw * s.cin / 64;
@@ -1642,7 +1038,7 @@ size_t conv_wgrad_workspace_bytes(const ConvShape& s) {
   return static_cast<size_t>(conv_wgrad_splits(s)) * s.kh * s.kw * s.cin * s.cout * sizeof(float);
 }
 
-// partial[split][(r,s,c)][cout] = sum over the split's pixels of X_gathered^T dY
+// partial[split][cout][(r,s,c)] = sum over the split's pixels of X_gathered^T dY
 int conv_wgrad_partials(const __nv_bfloat16* x, const __nv_bfloat16* dy, float* partial, const ConvShape& s, bool stem,
                         int* splits_out, cudaStream_t st) {
   if (int rc = check_shape(s, stem, "conv_wgrad")) return rc;
@@ -1659,25 +1055,6 @@ int conv_wgrad_partials(const __nv_bfloat16* x, const __nv_bfloat16* dy, float* 
   const int splits = conv_wgrad_splits(s);
   P.kblocks_per_split = (P.num_kblocks + splits - 1) / splits;
   P.ldc = s.cout; P.out = partial;
-  if (!stem) {
-    if (const int pr = patch_rows(s.h, s.w, s.cin, s.kh, s.kw, s.stride, s.pad, s.cout)) {
-      CUtensorMap tx, tdy;
-      if (int rc = make_tmap_patch(&tx, x, s.n, s.h, s.w, pr + 2)) return rc;
-      if (int rc = make_tmap_patch(&tdy, dy, s.n, s.ho, s.wo, pr)) return rc;
-      P.patch_r = pr; P.patch_wp = s.w + 2; P.patch_h = s.h; P.patch_w = s.w;
-      P.m_tiles = s.n * (s.h / pr);
-      const IgemmParams Q = finish_params(P);
-      static bool configured = false;
-      if (!configured) {
-        DIRB_CUDA(cudaFuncSetAttribute(wgrad_patch_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, kWgpSmemBytes));
-        configured = true;
-      }
-      *splits_out = splits;
-      wgrad_patch_kernel<<<splits, kWgpThreads, kWgpSmemBytes, st>>>(tx, tdy, Q);
-      DIRB_LAUNCHED();
-      return DIRB200_OK;
-    }
-  }
   const int bn = wgrad_bn(s);
   P.n_tiles = s.cout / bn;
   const int m_tiles = (P.total_chunks + 1) / 2;
@@ -1704,10 +1081,10 @@ int conv_wgrad_partials(const __nv_bfloat16* x, const __nv_bfloat16* dy, float* 
   return DISPATCH_BN(bn, true, false, tm, P, m_tiles, splits, st);
 }
 
-// Host-only description of the launch a conv would get (no CUDA call): which tile width, operand feeding form, CTA pairs
-// and split-K factor the selection logic above picks.  op: 0 fprop, 1 dgrad, 2 wgrad.
-// plan[0] = BN, plan[1] = 1 if CTA pairs, plan[2] = A-operand form (0 cp.async gather, 1 tiled TMA, 2 im2col TMA,
-// 3 patch-resident), plan[3] = rows per tile of the patch form (else 0), plan[4] = split-K factor (wgrad; else 1),
+// Host-only description of the launch a conv would get (no CUDA call): which tile width, operand feeding form and
+// split-K factor the selection logic above picks.  op: 0 fprop, 1 dgrad, 2 wgrad.
+// plan[0] = BN, plan[1] = 0 (no CTA pairs in this build), plan[2] = A-operand form (0 cp.async gather, 1 tiled TMA,
+// 2 im2col TMA), plan[3] = 0 (no patch-resident form in this build), plan[4] = split-K factor (wgrad; else 1),
 // plan[5] = launches (stride-2 dgrad: one per non-empty parity class), plan[6] = 1 if the dgrad can carry the BN-backward
 // moments of the previous layer.
 int conv_plan(const ConvShape& s, bool stem, int op, int* plan) {
@@ -1717,20 +1094,15 @@ int conv_plan(const ConvShape& s, bool stem, int op, int* plan) {
   if (op == 2) {
     plan[0] = wgrad_bn(s);
     plan[4] = conv_wgrad_splits(s);
-    if (!stem && patch_rows(s.h, s.w, s.cin, s.kh, s.kw, s.stride, s.pad, s.cout)) {
-      plan[0] = 64; plan[2] = 3; plan[3] = patch_rows(s.h, s.w, s.cin, s.kh, s.kw, s.stride, s.pad, s.cout);
-    } else if (stem) {
-      plan[2] = 0;
-    } else {
-      plan[2] = is_plain_gemm(s, stem) ? 1 : (im2col_enabled() ? 2 : 0);
-    }
+    plan[2] = stem ? 0 : (is_plain_gemm(s, stem) ? 1 : (im2col_enabled() ? 2 : 0));
     return DIRB200_OK;
   }
   const bool dgrad = op == 1;
   DIRB_CHECK_ARG(!(dgrad && stem), "conv_plan: the stem has no data gradient");
-  const int n_dim = dgrad ? s.cin : s.cout, k_ch = dgrad ? s.cout : s.cin;
+  const int n_dim = dgrad ? s.cin : s.cout;
+  plan[0] = pick_bn(n_dim);
   if (dgrad && s.stride == 2) {
-    int launches = 0, bn = 64;
+    int launches = 0;
     for (int cls = 0; cls < 4; ++cls) {
       const int py = cls >> 1, px = cls & 1;
       int nt = 0;
@@ -1740,26 +1112,12 @@ int conv_plan(const ConvShape& s, bool stem, int op, int* plan) {
       const int hm = (s.h - py + 1) / 2, wm = (s.w - px + 1) / 2;
       if (nt == 0 || hm <= 0 || wm <= 0) continue;
       ++launches;
-      const long long pixels = static_cast<long long>(s.n) * hm * wm;
-      bn = pick_bn(s.cin, (pixels + BM - 1) / BM, true);
     }
-    plan[0] = bn; plan[2] = im2col_enabled() ? 2 : 0; plan[5] = launches;
+    plan[2] = im2col_enabled() ? 2 : 0; plan[5] = launches;
     return DIRB200_OK;
   }
-  const int gh = dgrad ? s.ho : s.h, gw = dgrad ? s.wo : s.w;
-  if (!stem) {
-    if (const int pr = patch_rows(gh, gw, k_ch, s.kh, s.kw, s.stride, s.pad, n_dim)) {
-      plan[0] = 64; plan[2] = 3; plan[3] = pr; plan[6] = dgrad && conv_dgrad_fuses_bn_moments(s);
-      return DIRB200_OK;
-    }
-  }
-  const long long pixels = dgrad ? static_cast<long long>(s.n) * s.h * s.w : static_cast<long long>(s.n) * s.ho * s.wo;
-  const long long m_tiles = (pixels + BM - 1) / BM;
-  const int bn = pick_bn(n_dim, m_tiles, !is_plain_gemm(s, stem));
   const bool tma_fed = is_plain_gemm(s, stem) || (!stem && im2col_enabled() && (!dgrad || s.kh == s.kw));
-  plan[0] = bn;
   plan[2] = stem ? 0 : (is_plain_gemm(s, stem) ? 1 : (tma_fed ? 2 : 0));
-  plan[1] = tma_fed && want_pairs(bn, s.kh * s.kw * k_ch / 64);
   plan[6] = dgrad && conv_dgrad_fuses_bn_moments(s);
   return DIRB200_OK;
 }

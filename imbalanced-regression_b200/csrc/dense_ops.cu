@@ -1,7 +1,7 @@
 // Dense-prediction ops of the NYUD2-DIR model around the convolutions (SURVEY §8f-2), NHWC bf16:
 //   F.upsample(x, size, mode='bilinear')  (nyud2-dir/models/modules.py:24: align_corners = False)  forward + backward
 //   torch.cat(..., 1)                      (modules.py:120: channel concat of the four MFF branches)  = a strided copy
-// The convolutions themselves (5x5 / 3x3 / 1x1) are the tcgen05 implicit-GEMM kernels of conv_igemm.cu.
+// The convolutions themselves (5x5 / 3x3 / 1x1) are the wgmma implicit-GEMM kernels of conv_igemm.cu.
 #include "common.cuh"
 
 namespace dirb200 {

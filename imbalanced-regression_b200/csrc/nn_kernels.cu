@@ -1,4 +1,4 @@
-// HBM-bound layers of the ResNet stack around the tcgen05 convolutions, NHWC bf16:
+// HBM-bound layers of the ResNet stack around the wgmma convolutions, NHWC bf16:
 // batch-norm (training statistics, apply(+residual)(+ReLU), backward), 3x3/2 max-pool,
 // global average pool, the 2048->1 regressor and the fused Adam / SGD step.
 // Replaces nn.BatchNorm2d / nn.ReLU / nn.MaxPool2d / nn.AvgPool2d / nn.Linear of
@@ -234,8 +234,7 @@ __device__ __forceinline__ uint32_t f2_to_bf2(float a, float b) {
 // mask_out (block outputs only): one byte per (row, channel group): bit j = out[row][cg*8 + j] > 0 -- the ReLU mask
 // the backward kernels need, 1/16 of the size of `out`.
 // Rows per iteration R (4 for the plain form, 2 with a residual): every load of all R rows is issued before the first
-// use -- with one row per iteration the kernel sat at 5.1 TB/s (ncu launch list), the backward kernels with the same
-// structure and 2-4 rows in flight reach 6-6.7 TB/s.
+// use, so that several 16-byte loads per thread are in flight to cover the HBM latency (R has not been re-tuned on H100).
 template <bool HAS_RES, bool HAS_RESY, bool MASK>
 __global__ void __launch_bounds__(256)
 bn_apply_kernel(const __nv_bfloat16* __restrict__ y, const float* __restrict__ scale, const float* __restrict__ shift,
@@ -488,8 +487,8 @@ bn_bwd_apply_kernel(const __nv_bfloat16* __restrict__ g1, const __nv_bfloat16* _
                     const uint8_t* __restrict__ mask, int64_t rows, int c, __nv_bfloat16* __restrict__ dy,
                     __nv_bfloat16* __restrict__ dy2, __nv_bfloat16* __restrict__ dz_out) {
   // rows per iteration: every load of all of them is issued before the first use.  Two CTAs of 8 warps fit per SM
-  // (register-limited), so the plain two-input form needs four rows (8 x 16 B per thread) in flight to cover the HBM
-  // latency -- with two it ran at 4.4 TB/s (ncu, profiles/r2_bn_full.md); the forms with more inputs keep two.
+  // (register-limited), so the plain two-input form keeps four rows (8 x 16 B per thread) in flight to cover the HBM
+  // latency; the forms with more inputs keep two (not re-tuned on H100).
   constexpr bool HAS_G2 = G2M != G2_NONE;
   constexpr int R = (HAS_G2 || HAS_Y2) ? 2 : 4;
   const int cgroups = c / 8;

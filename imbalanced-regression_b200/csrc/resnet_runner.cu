@@ -1,5 +1,5 @@
 // Native runner of the bottleneck-ResNet backbone (agedb-dir/resnet.py:41-70,73-138): sequences the
-// tcgen05 convolutions and the HBM-bound layers for one forward and one backward pass over a fixed
+// wgmma convolutions and the HBM-bound layers for one forward and one backward pass over a fixed
 // batch shape, owning every activation / gradient / operand buffer (NHWC bf16) so that a training
 // step issues no allocation and no host synchronisation.
 //
@@ -383,8 +383,8 @@ static int forward_eval_folded(dirb200_net* net, const float* params, const floa
 }
 
 // The fixed-pointer launch sequences of a training step (~390 of its ~410 launches) are replayed as CUDA graphs (see
-// GraphSlot): the dependent-launch gaps of a stream, ~2 us each, were 0.8 ms of an 18.4 ms step (measured A/B on one
-// box: 18.36 -> 17.5 ms, end to end 18.48 -> 17.49 ms).  DIRB200_GRAPH=0 launches everything eagerly.
+// GraphSlot), which removes the dependent-launch gaps of a stream (A/B on an H100 80GB HBM3 at a 400 W power limit,
+// bench.py batch 256, two runs each: 41.6 ms per step with graphs, 42.1 ms eager).  DIRB200_GRAPH=0 launches eagerly.
 static bool graphs_enabled() {
   static const bool on = [] {
     const char* e = getenv("DIRB200_GRAPH");

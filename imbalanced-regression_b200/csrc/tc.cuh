@@ -1,6 +1,6 @@
-// Blackwell (sm_100a) primitives used by the implicit-GEMM convolution:
-// mbarrier, TMA (cp.async.bulk.tensor), cp.async, tcgen05 (alloc / mma / commit / ld),
-// UMMA shared-memory and instruction descriptors.  Inline PTX only.
+// Hopper (sm_90a) primitives used by the implicit-GEMM convolution:
+// mbarrier, TMA (cp.async.bulk.tensor), cp.async, wgmma (warpgroup MMA from shared memory, fp32 accumulators in
+// registers) and the wgmma shared-memory descriptor.  Inline PTX only.
 #pragma once
 #include <cuda.h>
 #include <stdint.h>
@@ -50,10 +50,9 @@ __device__ __forceinline__ void mbar_wait(uint32_t bar, uint32_t parity) {
   }
 }
 
-// One lane of the (fully converged) warp: the single-thread issue of TMA / tcgen05 instructions.  Issuing from
+// One lane of the (fully converged) warp: the single-thread issue of TMA instructions.  Issuing from
 // `if (elect_one())` in a CONVERGED warp -- rather than from a divergent `if (lane == 0)` region -- lets the compiler
-// keep descriptors / coordinates in uniform registers; in a divergent region every UTCHMMA / UTMALDG is wrapped in
-// an ELECT + R2UR.BROADCAST "uniformisation" loop (~15 instructions per MMA; measured cost on the conv GEMMs: 2-3 %).
+// keep descriptors / coordinates in uniform registers.
 __device__ __forceinline__ bool elect_one() {
   uint32_t pred;
   asm volatile(
@@ -70,17 +69,12 @@ __device__ __forceinline__ bool elect_one() {
 __device__ __forceinline__ void cp_async16(uint32_t dst, const void* src, uint32_t src_bytes) {
   asm volatile("cp.async.cg.shared.global [%0], [%1], 16, %2;" ::"r"(dst), "l"(src), "r"(src_bytes) : "memory");
 }
-__device__ __forceinline__ void cp_async_commit() { asm volatile("cp.async.commit_group;" ::: "memory"); }
-template <int N>
-__device__ __forceinline__ void cp_async_wait() {
-  asm volatile("cp.async.wait_group %0;" ::"n"(N) : "memory");
-}
 // arrive on `bar` once every cp.async previously issued by this thread has completed (does not raise the
 // barrier's pending count: the thread's arrival is part of the barrier's expected count)
 __device__ __forceinline__ void cp_async_mbar_arrive_noinc(uint32_t bar) {
   asm volatile("cp.async.mbarrier.arrive.noinc.shared::cta.b64 [%0];" ::"r"(bar) : "memory");
 }
-// generic-proxy smem writes -> visible to the async proxy (tcgen05.mma / TMA)
+// generic-proxy smem writes (cp.async, st.shared) -> visible to the async proxy (wgmma operand reads / TMA)
 __device__ __forceinline__ void fence_proxy_async() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
 
 // --------------------------------------------------------------------- TMA
@@ -88,16 +82,6 @@ __device__ __forceinline__ void tma_load_2d(uint32_t dst, const CUtensorMap* tma
   asm volatile(
       "cp.async.bulk.tensor.2d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4}], [%2];"
       ::"r"(dst), "l"(tmap), "r"(bar), "r"(c0), "r"(c1)
-      : "memory");
-}
-
-// tiled-mode 4-D load (NHWC tensor as C, W, H, N): a box starting at (c, w, h, n); coordinates may be negative /
-// past the extent, out-of-range elements arrive as zeros (the conv padding)
-__device__ __forceinline__ void tma_load_4d(uint32_t dst, const CUtensorMap* tmap, uint32_t bar, int c, int w, int h,
-                                            int n) {
-  asm volatile(
-      "cp.async.bulk.tensor.4d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4, %5, %6}], [%2];"
-      ::"r"(dst), "l"(tmap), "r"(bar), "r"(c), "r"(w), "r"(h), "r"(n)
       : "memory");
 }
 
@@ -113,127 +97,63 @@ __device__ __forceinline__ void tma_load_im2col_4d(uint32_t dst, const CUtensorM
       : "memory");
 }
 
-// ------------------------------------------------------------------ tcgen05
-__device__ __forceinline__ void tmem_alloc(uint32_t holder_smem, uint32_t ncols) {
-  asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(holder_smem), "r"(ncols)
-               : "memory");
-  asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
+// ------------------------------------------------------------------- wgmma
+// A warpgroup (4 consecutive warps, the first one a multiple of 4) computes D[64 x N] (+)= A[64 x 16] * B[16 x N]
+// with both operands in shared memory.  Accumulator fragment of thread t (warp w = (t / 32) % 4, lane l = t % 32):
+// d[4j + e] (e = 0, 1) is row 16w + l/4, column 8j + 2(l%4) + e; d[4j + 2 + e] the same columns of row 16w + l/4 + 8.
+__device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+template <int N>
+__device__ __forceinline__ void wgmma_wait() {
+  asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory");
 }
-__device__ __forceinline__ void tmem_dealloc(uint32_t taddr, uint32_t ncols) {
-  asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(ncols) : "memory");
-}
-__device__ __forceinline__ void tcgen05_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tcgen05_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
-
-// D[tmem] (+)= A[smem] * B[smem], bf16 inputs, fp32 accumulate, one CTA.
-__device__ __forceinline__ void umma_bf16(uint32_t tmem_d, uint64_t adesc, uint64_t bdesc, uint32_t idesc,
-                                          uint32_t accumulate) {
-  asm volatile(
-      "{\n"
-      ".reg .pred p;\n"
-      "setp.ne.b32 p, %4, 0;\n"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n"
-      "}\n" ::"r"(tmem_d),
-      "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-// mbarrier arrives once all previously issued tcgen05.mma of this thread have completed
-__device__ __forceinline__ void umma_commit(uint32_t bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(bar) : "memory");
+// keeps the compiler from moving accumulator accesses across the asynchronous MMAs
+template <int R>
+__device__ __forceinline__ void wgmma_fence_operands(float (&d)[R]) {
+#pragma unroll
+  for (int i = 0; i < R; ++i) asm volatile("" : "+f"(d[i])::"memory");
 }
 
-// ------------------------------------------------ CTA pair (cta_group::2) primitives
-// Two CTAs of a (2,1,1) cluster run one UMMA of M = 256: each CTA holds its own 128 rows of A and HALF of B in shared
-// memory at identical offsets and its own 128 accumulator lanes in TMEM; the even CTA ("leader") issues the MMAs.
-__device__ __forceinline__ uint32_t cluster_ctarank() {
-  uint32_t r;
-  asm volatile("mov.u32 %0, %%cluster_ctarank;" : "=r"(r));
-  return r;
-}
-__device__ __forceinline__ void cluster_sync_all() {
-  asm volatile("barrier.cluster.arrive.release.aligned;" ::: "memory");
-  asm volatile("barrier.cluster.wait.acquire.aligned;" ::: "memory");
-}
-// shared::cluster address of `local_addr` (a shared::cta address of this CTA) in CTA `rank` of the cluster
-__device__ __forceinline__ uint32_t mapa_rank(uint32_t local_addr, uint32_t rank) {
-  uint32_t r;
-  asm volatile("mapa.shared::cluster.u32 %0, %1, %2;" : "=r"(r) : "r"(local_addr), "r"(rank));
-  return r;
-}
-// Arrive on a barrier of another CTA of the cluster.  Default (.release.cta) semantics as cutlass::arch::ClusterBarrier
-// does: the explicit .release.cluster form compiles to MEMBAR.ALL.GPU + ERRBAR in front of every arrive (measured: the
-// per-k-block relay then throttles the whole pair).  What is handed over here is never read through this thread's
-// generic loads: gathered rows sit in the peer's own shared memory (written before its local barrier completed) and
-// TMEM reads are ordered by tcgen05.wait::ld + tcgen05.fence::before_thread_sync.
-__device__ __forceinline__ void mbar_arrive_remote(uint32_t cluster_addr) {
-  asm volatile("mbarrier.arrive.shared::cluster.b64 _, [%0];" ::"r"(cluster_addr) : "memory");
-}
-// TMA load into THIS CTA's smem whose transaction bytes are counted on the LEADER CTA's mbarrier (same offset, peer
-// bit cleared), as cute::SM100_TMA_2SM_LOAD_2D does
-__device__ __forceinline__ void tma_load_2d_cta2(uint32_t dst, const CUtensorMap* tmap, uint32_t bar, int c0, int c1) {
+// TA / TB: 0 = the operand is K-major, 1 = MN-major (transposed); accumulate = 0 overwrites D.
+#define DIRB_F4(i) "+f"(d[i]), "+f"(d[i + 1]), "+f"(d[i + 2]), "+f"(d[i + 3])
+#define DIRB_F16(i) DIRB_F4(i), DIRB_F4(i + 4), DIRB_F4(i + 8), DIRB_F4(i + 12)
+#define DIRB_R8(a, b, c, e, f, g, h, k) "%" #a ", %" #b ", %" #c ", %" #e ", %" #f ", %" #g ", %" #h ", %" #k ", "
+template <int TA, int TB>
+__device__ __forceinline__ void wgmma_m64n64(float (&d)[32], uint64_t adesc, uint64_t bdesc, uint32_t accumulate) {
   asm volatile(
-      "cp.async.bulk.tensor.2d.cta_group::2.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4}], [%2];"
-      ::"r"(dst), "l"(tmap), "r"(bar & 0xFEFFFFFFu), "r"(c0), "r"(c1)
-      : "memory");
+      "{\n.reg .pred p;\nsetp.ne.b32 p, %34, 0;\n"
+      "wgmma.mma_async.sync.aligned.m64n64k16.f32.bf16.bf16 {"
+      DIRB_R8(0, 1, 2, 3, 4, 5, 6, 7) DIRB_R8(8, 9, 10, 11, 12, 13, 14, 15) DIRB_R8(16, 17, 18, 19, 20, 21, 22, 23)
+      "%24, %25, %26, %27, %28, %29, %30, %31}, %32, %33, p, 1, 1, %35, %36;\n}\n"
+      : DIRB_F16(0), DIRB_F16(16)
+      : "l"(adesc), "l"(bdesc), "r"(accumulate), "n"(TA), "n"(TB));
 }
-// im2col-mode variant of the above (cute::SM100_TMA_2SM_LOAD_IM2COL_4D)
-__device__ __forceinline__ void tma_load_im2col_4d_cta2(uint32_t dst, const CUtensorMap* tmap, uint32_t bar, int c, int w,
-                                                        int h, int n, uint16_t off_w, uint16_t off_h) {
+template <int TA, int TB>
+__device__ __forceinline__ void wgmma_m64n128(float (&d)[64], uint64_t adesc, uint64_t bdesc, uint32_t accumulate) {
   asm volatile(
-      "cp.async.bulk.tensor.4d.im2col.cta_group::2.shared::cluster.global.mbarrier::complete_tx::bytes"
-      " [%0], [%1, {%3, %4, %5, %6}], [%2], {%7, %8};"
-      ::"r"(dst), "l"(tmap), "r"(bar & 0xFEFFFFFFu), "r"(c), "r"(w), "r"(h), "r"(n), "h"(off_w), "h"(off_h)
-      : "memory");
+      "{\n.reg .pred p;\nsetp.ne.b32 p, %66, 0;\n"
+      "wgmma.mma_async.sync.aligned.m64n128k16.f32.bf16.bf16 {"
+      DIRB_R8(0, 1, 2, 3, 4, 5, 6, 7) DIRB_R8(8, 9, 10, 11, 12, 13, 14, 15) DIRB_R8(16, 17, 18, 19, 20, 21, 22, 23)
+      DIRB_R8(24, 25, 26, 27, 28, 29, 30, 31) DIRB_R8(32, 33, 34, 35, 36, 37, 38, 39) DIRB_R8(40, 41, 42, 43, 44, 45, 46, 47)
+      DIRB_R8(48, 49, 50, 51, 52, 53, 54, 55)
+      "%56, %57, %58, %59, %60, %61, %62, %63}, %64, %65, p, 1, 1, %67, %68;\n}\n"
+      : DIRB_F16(0), DIRB_F16(16), DIRB_F16(32), DIRB_F16(48)
+      : "l"(adesc), "l"(bdesc), "r"(accumulate), "n"(TA), "n"(TB));
 }
-__device__ __forceinline__ void tmem_alloc_cta2(uint32_t holder_smem, uint32_t ncols) {
-  asm volatile("tcgen05.alloc.cta_group::2.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(holder_smem), "r"(ncols)
-               : "memory");
-  asm volatile("tcgen05.relinquish_alloc_permit.cta_group::2.sync.aligned;" ::: "memory");
+#undef DIRB_R8
+#undef DIRB_F16
+#undef DIRB_F4
+// D (+)= A * B for a 64 x BN warpgroup tile, BN = 64 or 128
+template <int BN, int TA, int TB>
+__device__ __forceinline__ void wgmma_bf16(float (&d)[BN / 2], uint64_t adesc, uint64_t bdesc, uint32_t accumulate) {
+  if constexpr (BN == 128) wgmma_m64n128<TA, TB>(d, adesc, bdesc, accumulate);
+  else wgmma_m64n64<TA, TB>(d, adesc, bdesc, accumulate);
 }
-__device__ __forceinline__ void tmem_dealloc_cta2(uint32_t taddr, uint32_t ncols) {
-  asm volatile("tcgen05.dealloc.cta_group::2.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(ncols) : "memory");
-}
-// D[tmem of both CTAs] (+)= A * B over the CTA pair (M = 256); issued by one thread of the leader CTA only
-__device__ __forceinline__ void umma_bf16_cta2(uint32_t tmem_d, uint64_t adesc, uint64_t bdesc, uint32_t idesc,
-                                               uint32_t accumulate) {
-  const uint32_t z = 0u;
-  asm volatile(
-      "{\n"
-      ".reg .pred p;\n"
-      "setp.ne.b32 p, %4, 0;\n"
-      "tcgen05.mma.cta_group::2.kind::f16 [%0], %1, %2, %3, {%5, %5, %5, %5, %5, %5, %5, %5}, p;\n"
-      "}\n" ::"r"(tmem_d),
-      "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate), "r"(z)
-      : "memory");
-}
-// the barrier at this offset in BOTH CTAs of the pair receives one arrival when the pair's MMAs issued so far are done
-__device__ __forceinline__ void umma_commit_cta2(uint32_t bar) {
-  const uint16_t mask = 3;
-  asm volatile(
-      "tcgen05.commit.cta_group::2.mbarrier::arrive::one.shared::cluster.multicast::cluster.b64 [%0], %1;" ::"r"(bar),
-      "h"(mask)
-      : "memory");
-}
-
-// 32 lanes x 32 columns of fp32 accumulators -> 32 registers per thread
-__device__ __forceinline__ void tmem_ld_32x32(uint32_t taddr, uint32_t (&v)[32]) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-      : "=r"(v[0]), "=r"(v[1]), "=r"(v[2]), "=r"(v[3]), "=r"(v[4]), "=r"(v[5]), "=r"(v[6]), "=r"(v[7]), "=r"(v[8]),
-        "=r"(v[9]), "=r"(v[10]), "=r"(v[11]), "=r"(v[12]), "=r"(v[13]), "=r"(v[14]), "=r"(v[15]), "=r"(v[16]),
-        "=r"(v[17]), "=r"(v[18]), "=r"(v[19]), "=r"(v[20]), "=r"(v[21]), "=r"(v[22]), "=r"(v[23]), "=r"(v[24]),
-        "=r"(v[25]), "=r"(v[26]), "=r"(v[27]), "=r"(v[28]), "=r"(v[29]), "=r"(v[30]), "=r"(v[31])
-      : "r"(taddr)
-      : "memory");
-}
-__device__ __forceinline__ void tmem_ld_wait() { asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory"); }
 
 // ------------------------------------------------------------- descriptors
-// Shared-memory matrix descriptor, SWIZZLE_128B (layout_type 2), descriptor version 1 (sm_100).
+// wgmma shared-memory matrix descriptor, 128-byte swizzle (layout type 1, bits [62,64)):
 //   bits [0,14)  start address >> 4        bits [16,30) leading byte offset >> 4
-//   bits [32,46) stride byte offset >> 4   bits [46,48) version = 1      bits [61,64) layout type
+//   bits [32,46) stride byte offset >> 4   bits [49,52) base offset = 0 (tiles start 1024-byte aligned)
 // K-major tile  [rows][64 bf16]: rows 128 B apart, 8-row atoms 1024 B apart  -> SBO = 1024, LBO unused.
 // MN-major tile [chunk][k rows][64 bf16 of M/N]: k rows 128 B apart, 8-k atoms 1024 B apart (SBO),
 //               64-wide M/N chunks `lbo_bytes` apart (LBO).
@@ -242,18 +162,8 @@ __device__ __forceinline__ uint64_t make_smem_desc(uint32_t saddr, uint32_t lbo_
   d |= static_cast<uint64_t>((saddr & 0x3FFFFu) >> 4);
   d |= static_cast<uint64_t>((lbo_bytes >> 4) & 0x3FFFu) << 16;
   d |= static_cast<uint64_t>((sbo_bytes >> 4) & 0x3FFFu) << 32;
-  d |= static_cast<uint64_t>(1) << 46;
-  d |= static_cast<uint64_t>(2) << 61;
+  d |= static_cast<uint64_t>(1) << 62;
   return d;
-}
-
-// Instruction descriptor for kind::f16: fp32 accumulate, bf16 A and B.
-//   [4,6) c_format=1(F32)  [7,10) a_format=1(BF16)  [10,13) b_format=1(BF16)
-//   [15] a_major (0 = K, 1 = MN)  [16] b_major  [17,23) N>>3  [24,29) M>>4
-__host__ __device__ constexpr uint32_t make_idesc(int m, int n, int a_mn_major, int b_mn_major) {
-  return (1u << 4) | (1u << 7) | (1u << 10) | (static_cast<uint32_t>(a_mn_major) << 15) |
-         (static_cast<uint32_t>(b_mn_major) << 16) | (static_cast<uint32_t>(n >> 3) << 17) |
-         (static_cast<uint32_t>(m >> 4) << 24);
 }
 
 }  // namespace tc

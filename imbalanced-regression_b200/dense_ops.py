@@ -1,8 +1,8 @@
 """dense_ops.py -- the operators of the NYUD2-DIR decoder / feature-fusion / refinement modules
-(nyud2-dir/models/modules.py:6-174) on the B200 path, as autograd functions over NHWC bf16 tensors:
+(nyud2-dir/models/modules.py:6-174) on the native path, as autograd functions over NHWC bf16 tensors:
 
   conv2d_nhwc(x, weight, stride, padding)   nn.Conv2d(..., bias=False) with 1x1 / 3x3 / 5x5 filters (modules.py:11-20, 63,
-                                            107, 134-141): tcgen05 implicit GEMM, forward + data / weight gradients
+                                            107, 134-141): wgmma implicit GEMM, forward + data / weight gradients
   upsample_bilinear(x, size)                F.upsample(x, size=size, mode='bilinear') (modules.py:24)
   cat_channels(tensors)                     torch.cat(tensors, 1) (modules.py:120)
   batch_norm_train(x, weight, bias, ...)    nn.BatchNorm2d in training mode [+ ReLU] (modules.py:13-21, 65, 109, 137-141)

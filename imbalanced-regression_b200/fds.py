@@ -1,5 +1,5 @@
 """fds.FDS -- drop-in mirror of the reference module (agedb-dir/fds.py:14-144,
-imdb-wiki-dir/fds.py) whose arithmetic runs in libdirb200's sm_100a kernels.
+imdb-wiki-dir/fds.py) whose arithmetic runs in libdirb200's sm_90a kernels.
 
 Same constructor, same eight registered buffers (identical state_dict keys and
 shapes, fds.py:28-35), same methods and state machine -- including the

@@ -7,7 +7,7 @@ linear, FDS), hence the reference's state_dict keys and shapes, the same
 same initialisation (resnet.py:103-109).
 
 The arithmetic does not go through torch.nn: the conv/BN/ReLU/pool stack runs
-in libdirb200's native runner (tcgen05 implicit-GEMM convolutions + fused
+in libdirb200's native runner (wgmma implicit-GEMM convolutions + fused
 HBM-bound layers, NHWC bf16 with fp32 accumulation), the 2048->1 regressor
 and FDS.smooth in their own kernels.  All parameters are views into ONE flat
 fp32 buffer (and their .grad into one flat gradient buffer), which is what the
@@ -155,7 +155,7 @@ class ResNet(nn.Module):
                  kernel, ks, sigma, momentum, dropout=None):
         self.inplanes = 64
         super(ResNet, self).__init__()
-        assert block is Bottleneck, "the B200 runner implements the bottleneck ResNets (resnet50 and deeper)"
+        assert block is Bottleneck, "the native runner implements the bottleneck ResNets (resnet50 and deeper)"
         self._layers = list(layers)
         self.conv1 = _Conv(3, 64, 7, 2, 3)
         self.bn1 = _BN(64)

@@ -1,6 +1,6 @@
 """train.py -- host driver mirroring agedb-dir/train.py / imdb-wiki-dir/train.py
 (same flags, same store-name rule, same train / validate / checkpoint flow)
-on top of the B200-native modules of this directory.
+on top of the H100-native modules of this directory.
 
 Differences that matter:
   * one process per GPU (`torchrun --nproc-per-node N train.py ...`): the

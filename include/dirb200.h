@@ -1,9 +1,9 @@
-/* dirb200.h -- C ABI of libdirb200.so: the B200-native (sm_100a) hot path of
+/* dirb200.h -- C ABI of libdirb200.so: the H100-native (sm_90a) hot path of
  * YyzHarry/imbalanced-regression (ResNet-50 + FDS + LDS training step).
  *
  * The reference has no FFI: its "plugin boundary" for this path is a set of
  * Python callables (SURVEY.md §8b).  Each entry point below names the
- * reference function it replaces (file:line under /root/reference); the
+ * reference function it replaces (file:line in the reference repository); the
  * Python host mirrors in imbalanced-regression_b200/{fds,loss,utils,resnet,
  * datasets}.py keep the reference's names/signatures and call these through
  * ctypes (see INTEGRATION.md).
@@ -232,7 +232,7 @@ int dirb200_shot_metrics(const float* preds, const float* labels, int64_t n, con
  * [Cout][Cin][KH][KW] layout (agedb-dir/resnet.py:46-51,79,112-118, i.e. the
  * nn.Conv2d parameters / state_dict tensors) and are re-laid-out to bf16 GEMM
  * operands by dirb200_conv_prep_weights.  The convolutions themselves are
- * tcgen05 implicit GEMMs (fp32 accumulate in TMEM); they replace the cuDNN
+ * wgmma implicit GEMMs (fp32 accumulate in registers); they replace the cuDNN
  * calls behind nn.Conv2d forward and its autograd backward.
  * Cin and Cout must be multiples of 64, except the stem (stem=1: Cin=3, 7x7,
  * stride 2, pad 3), which consumes the 16-channel space-to-depth input made
@@ -256,9 +256,9 @@ int dirb200_conv_dgrad(const void* dy, const void* w_dgrad, void* dx, int n, int
                        int cout, int kh, int kw, int stride, int pad, void* stream);
 
 /* Host-only (no CUDA call, works without a device): which GEMM form the three entry points above / below would launch for
- * a shape (op: 0 fprop, 1 dgrad, 2 wgrad).  plan7[0] tile width BN; [1] 1 = CTA pairs (cta_group::2); [2] A-operand form:
- * 0 cp.async gather, 1 tiled TMA, 2 im2col-mode TMA, 3 patch-resident (one input patch in shared memory, taps as
- * displaced descriptors); [3] image rows per tile of the patch form; [4] split-K factor (wgrad); [5] launches (a stride-2
+ * a shape (op: 0 fprop, 1 dgrad, 2 wgrad).  plan7[0] tile width BN; [1] 0 (no CTA pairs on
+ * sm_90a); [2] A-operand form: 0 cp.async gather, 1 tiled TMA, 2 im2col-mode TMA; [3] 0 (no patch-resident form on
+ * sm_90a); [4] split-K factor (wgrad); [5] launches (a stride-2
  * dgrad runs one per non-empty output-pixel parity class); [6] 1 = this dgrad can also accumulate the BN-backward
  * moments of the previous layer in its epilogue. */
 int dirb200_conv_plan(int n, int h, int w, int cin, int cout, int kh, int kw, int stride, int pad, int stem, int op,

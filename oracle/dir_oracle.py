@@ -9,7 +9,7 @@ Each function is an independent numpy restatement of the reference algorithm
 (YyzHarry/imbalanced-regression @ a6fdc45) and cites the reference lines it
 follows.  The restatement is pinned against the reference itself: the
 fixtures in `tests/golden/*.npz` were produced by importing the reference's
-own modules from `/root/reference` (see `tests/golden/make_golden.py`) and
+own modules (see `tests/golden/make_golden.py`) and
 `tests/test_oracle_golden.py` checks this file against them.  The reference
 ships no tests / golden vectors of its own (SURVEY.md §4), so this is the
 strongest pin available.

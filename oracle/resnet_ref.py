@@ -1,6 +1,6 @@
 """Plain-PyTorch fp32 restatement of the reference ResNet-50 regressor
 (agedb-dir/resnet.py:41-70 Bottleneck, :73-153 ResNet) as pure functions over a
-state_dict -- TEST INFRASTRUCTURE ONLY (the checker for the bf16 tcgen05 conv
+state_dict -- TEST INFRASTRUCTURE ONLY (the checker for the bf16 wgmma conv
 stack; see oracle/dir_oracle.py for the rules).
 
 Pinned against the reference itself by tests/test_oracle_golden.py::test_resnet_ref
@@ -46,7 +46,7 @@ def _bn(x, p, pre, stats, quant):
 
 
 def _q(x, quant):
-    """bf16 round trip of a stored activation (what the B200 path keeps in HBM);
+    """bf16 round trip of a stored activation (what the native path keeps in HBM);
     straight-through in the backward."""
     if not quant:
         return x
@@ -55,7 +55,7 @@ def _q(x, quant):
 
 class _RoundBoth(torch.autograd.Function):
     """bf16 rounding of the value in the forward AND of the gradient in the
-    backward: the points where the B200 path stores a gradient tensor as bf16
+    backward: the points where the native path stores a gradient tensor as bf16
     (conv output grads dy, conv input grads from dgrad, the identity-branch dz,
     the avg-pool / max-pool input grads)."""
 
@@ -80,7 +80,7 @@ def _conv(x, w, stride, pad, quant):
 
 def forward_encoding(p, x, layers=LAYERS, stats=None, quant=False, taps=None, force=None):
     """x [B,3,H,W] -> encoding [B,2048]; train-mode BN.  quant=True mimics the
-    bf16 storage points of the B200 path (weights, conv outputs, activations)
+    bf16 storage points of the native path (weights, conv outputs, activations)
     with straight-through rounding, so tolerances can be tight."""
     def tap(name, t):
         # `force`: teacher forcing -- substitute the value of a stored activation (keeping the gradient path), so

@@ -2,8 +2,8 @@
 forward through ResNet-50 with FDS.smooth, weighted L1, backward, Adam) in
 plain PyTorch fp32 -- TEST INFRASTRUCTURE / CPU BASELINE ONLY (bench.py's
 `cpu_baseline` and `--impl reference` legs; see oracle/dir_oracle.py's header).
-It is the "port" kind of baseline: /root/reference (Python) cannot travel to
-the GPU box, so the timed CPU arm is this restatement, which uses the same
+It is the "port" kind of baseline: where no copy of the reference's own
+modules is installed (oracle/_ref), the timed CPU arm is this restatement, which uses the same
 torch CPU kernels (MKL-DNN convolutions, ATen BN/ReLU, autograd, torch.optim.Adam)
 the reference's own modules would dispatch to.
 """

@@ -1,6 +1,5 @@
 """Multi-GPU correctness on hardware (SURVEY.md section 4, "1-vs-2-vs-8 GPU equality"), run under torchrun on N GPUs of
-one box (not collected by pytest; tools/r2_call7.sh runs it with N = 2, the driver's scaling run covers N = 8 through
-bench.py's replica_check):
+one box (not collected by pytest; run it with torchrun on N = 2; bench.py's replica_check covers N = 8):
 
     python -m torch.distributed.run --nnodes=1 --nproc-per-node N --master-addr 127.0.0.1 tests/mgpu_check.py
 

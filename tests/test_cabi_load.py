@@ -48,12 +48,16 @@ def test_no_cpu_fallback():
 
 def test_wgrad_split_search_never_leaves_a_straggler_wave():
     """Host-side scheduling of the wgrad split-K GEMM (csrc/conv_igemm.cu: conv_wgrad_splits), observable without a
-    GPU through dirb200_conv_wgrad_workspace_bytes = splits * K_total * Cout * 4 (num_sms() falls back to 148 when no
-    device is present).  For every conv of the batch-256 ResNet-50: the work items (tiles x splits) must fill the
-    persistent CTAs' waves to >= 85 % -- the earlier ceil(2*SMs/tiles) rule left e.g. 297 items (a third wave for one
-    item) on the 3x3 layers -- and every split keeps >= 8 k-blocks."""
+    GPU through dirb200_conv_wgrad_workspace_bytes = splits * K_total * Cout * 4, with the SM count the library itself
+    uses (num_sms(): the device's, capped by DIRB200_SMS; the H100 SXM's 132 when no device is present).  For every conv of the batch-256 ResNet-50: the work items (tiles x splits) must fill the
+    persistent CTAs' waves to >= 85 % -- a ceil(2*SMs/tiles) rule leaves a straggler wave of a few items on the 3x3
+    layers -- and every split keeps >= 8 k-blocks."""
     import _lib, _convlib  # noqa: F401
-    sms = 148
+    import torch
+    sms = torch.cuda.get_device_properties(0).multi_processor_count if torch.cuda.is_available() else 132
+    cap = int(os.environ.get("DIRB200_SMS", "0") or 0)
+    if 0 < cap < sms:
+        sms = cap
     convs = []          # (h, cin, cout, k, stride, pad)
     h, inpl = 56, 64
     for li, nb in enumerate((3, 4, 6, 3)):
@@ -72,7 +76,7 @@ def test_wgrad_split_search_never_leaves_a_straggler_wave():
         assert splits >= 1 and nbytes == splits * k * k * cin * cout * 4
         ho = (hh + 2 * p - k) // s + 1
         kblocks = (256 * ho * ho + 63) // 64
-        bn = 256 if cout % 256 == 0 else (128 if cout % 128 == 0 else 64)
+        bn = 128 if cout % 128 == 0 else 64
         tiles = ((k * k * cin // 64 + 1) // 2) * (cout // bn)
         items = tiles * splits
         waves = -(-items // sms)
@@ -85,7 +89,7 @@ def test_wgrad_split_search_never_leaves_a_straggler_wave():
 
 def test_conv_plan_selects_the_intended_gemm_forms():
     """Host-only selection logic of the conv stage (dirb200_conv_plan; no device needed): the batch-256 ResNet-50 shapes
-    get the forms DESIGN.md section 4.1 describes."""
+    get the forms DESIGN.md section 4 describes."""
     import ctypes
     import _lib, _convlib  # noqa: F401
 
@@ -96,29 +100,29 @@ def test_conv_plan_selects_the_intended_gemm_forms():
         assert rc == 0, _lib.last_error()
         return dict(zip(("bn", "pairs", "feed", "patch_rows", "splits", "launches", "bn_moments"), a))
 
-    GATHER, TILED, IM2COL, PATCH = 0, 1, 2, 3
-    # layer1 conv2 (64 -> 64 3x3 at 56x56): patch-resident in all three passes, 2 padded rows per tile, one partial per CTA
+    GATHER, TILED, IM2COL = 0, 1, 2
+    # layer1 conv2 (64 -> 64 3x3 at 56x56): im2col TMA, 64-wide tiles in all three passes; its dgrad carries BN moments
     for op in (0, 1, 2):
         q = plan(56, 64, 64, 3, 1, 1, op)
-        assert (q["feed"], q["patch_rows"], q["bn"]) == (PATCH, 2, 64), q
-    assert plan(56, 64, 64, 3, 1, 1, 2)["splits"] == 148 and plan(56, 64, 64, 3, 1, 1, 1)["bn_moments"] == 1
-    # 1x1 stride-1 GEMMs: tiled TMA; K-heavy 256-wide ones as CTA pairs
-    assert plan(56, 64, 256, 1, 1, 0, 0) == dict(bn=256, pairs=0, feed=TILED, patch_rows=0, splits=1, launches=1, bn_moments=0)
+        assert (q["feed"], q["patch_rows"], q["bn"], q["pairs"]) == (IM2COL, 0, 64, 0), q
+    assert plan(56, 64, 64, 3, 1, 1, 1)["bn_moments"] == 1
+    # 1x1 stride-1 GEMMs: tiled TMA, 128-wide tiles wherever N allows (one m64n128 wgmma per consumer warpgroup)
+    assert plan(56, 64, 256, 1, 1, 0, 0) == dict(bn=128, pairs=0, feed=TILED, patch_rows=0, splits=1, launches=1, bn_moments=0)
     q = plan(14, 256, 1024, 1, 1, 0, 0)
-    assert (q["bn"], q["pairs"], q["feed"]) == (256, 1, TILED)
-    q = plan(7, 2048, 512, 1, 1, 0, 1)                   # dgrad: N = Cin = 2048 -> 256-wide pair tiles, carries BN moments
-    assert (q["bn"], q["pairs"], q["bn_moments"]) == (256, 1, 1)
-    # 3x3 layers: im2col TMA; pairs from layer3 on; stride-2 dgrad = 4 TMA-fed parity-class launches, no BN moments
+    assert (q["bn"], q["pairs"], q["feed"]) == (128, 0, TILED)
+    q = plan(7, 2048, 512, 1, 1, 0, 1)                   # dgrad: N = Cin = 2048, carries BN moments
+    assert (q["bn"], q["pairs"], q["bn_moments"]) == (128, 0, 1)
+    # 3x3 layers: im2col TMA; stride-2 dgrad = 4 TMA-fed parity-class launches, no BN moments
     q = plan(28, 128, 128, 3, 1, 1, 0)
     assert (q["bn"], q["pairs"], q["feed"]) == (128, 0, IM2COL)
     q = plan(14, 256, 256, 3, 1, 1, 0)
-    assert (q["bn"], q["pairs"], q["feed"]) == (256, 1, IM2COL)
+    assert (q["bn"], q["pairs"], q["feed"]) == (128, 0, IM2COL)
     q = plan(56, 128, 128, 3, 2, 1, 1)
     assert (q["feed"], q["launches"], q["bn_moments"]) == (IM2COL, 4, 0)
     q = plan(56, 256, 512, 1, 2, 0, 1)                   # 1x1 stride-2 downsample: only the (even, even) class has a tap
     assert q["launches"] == 1
-    # wgrad never runs as pairs; every split keeps work (checked in detail by the test above)
-    assert plan(14, 256, 256, 3, 1, 1, 2)["pairs"] == 0
+    # wgrad: split-K (checked in detail by the test above)
+    assert plan(14, 256, 256, 3, 1, 1, 2)["pairs"] == 0 and plan(14, 256, 256, 3, 1, 1, 2)["splits"] > 1
     # 5x5 (NYUD2 refinement conv) goes through im2col TMA as well; the stem keeps the cp.async gather
     assert plan(240, 128, 128, 5, 1, 2, 0)["feed"] == IM2COL
     assert plan(224, 3, 64, 7, 2, 3, 0, stem=1)["feed"] == GATHER

@@ -1,4 +1,4 @@
-"""GPU parity of the tcgen05 implicit-GEMM convolutions (fprop / dgrad / wgrad)
+"""GPU parity of the wgmma implicit-GEMM convolutions (fprop / dgrad / wgrad)
 against torch fp32 conv (TF32 off) on the same bf16-rounded operands.  Tolerance: the
 kernel accumulates in fp32 and rounds the result to bf16 once, so outputs must
 match the fp32 reference to bf16 precision (rel 2^-8 of the tensor scale);
@@ -98,20 +98,19 @@ def run_conv(n, h, w, cin, cout, k, stride, pad, seed=0, check_dgrad=True, devic
     (1, 14, 14, 1024, 256, 1, 1, 0),   # 16 k-blocks > ring depth
     (4, 7, 7, 512, 2048, 1, 1, 0),     # 16 n-tiles
     (5, 9, 11, 64, 128, 3, 2, 1),      # odd sizes, non-square
-    (75, 14, 14, 256, 256, 3, 1, 1),   # CTA pairs + im2col TMA: 115 m-tiles (odd: last pair has an empty peer half)
-    (64, 28, 28, 512, 256, 1, 1, 0),   # CTA pairs + tiled TMA: 392 m-tiles, 8 k-blocks
-    (64, 14, 14, 256, 1024, 1, 1, 0),  # CTA pairs, 4 n-tiles per cluster walk, accumulator double buffering
-    # patch-resident 3x3 form (64 -> 64, stride 1): tiles of r whole padded image rows, nine displaced descriptors
-    (3, 12, 20, 64, 64, 3, 1, 1),      # r = 4 rows of 22 padded columns (88 of 128 tile rows live), non-square
-    (5, 7, 9, 64, 64, 3, 1, 1),        # r = 7: one tile per image
-    (4, 56, 56, 64, 64, 3, 1, 1),      # the layer1 shape: r = 2 rows of 58, 112 tiles on 112 CTAs
-    (1, 6, 60, 64, 64, 3, 1, 1),       # widest supported row (62 padded columns): the last tap reads to the slot's end
-    (2, 5, 100, 64, 64, 3, 1, 1),      # too wide for a patch slot: im2col form
+    (75, 14, 14, 256, 256, 3, 1, 1),   # im2col TMA: 115 m-tiles, several tiles per CTA
+    (64, 28, 28, 512, 256, 1, 1, 0),   # tiled TMA: 392 m-tiles, 8 k-blocks
+    (64, 14, 14, 256, 1024, 1, 1, 0),  # 8 n-tiles, several tiles per CTA
+    (3, 12, 20, 64, 64, 3, 1, 1),      # non-square
+    (5, 7, 9, 64, 64, 3, 1, 1),
+    (4, 56, 56, 64, 64, 3, 1, 1),      # the layer1 shape
+    (1, 6, 60, 64, 64, 3, 1, 1),
+    (2, 5, 100, 64, 64, 3, 1, 1),
     # 5x5 / stride 1 / pad 2: the NYUD2 decoder and refinement convolutions (nyud2-dir/models/modules.py:11-20,154-160)
     (2, 12, 16, 128, 128, 5, 1, 2),    # R.conv0 / conv1 form: 25 taps x 2 channel blocks = 50 k-blocks
     (3, 9, 11, 64, 128, 5, 1, 2),      # odd sizes
     (1, 24, 32, 128, 64, 5, 1, 2),     # up-projection form (Cout < Cin)
-    (2, 8, 8, 256, 256, 5, 1, 2),      # CTA pairs with 100 k-blocks
+    (2, 8, 8, 256, 256, 5, 1, 2),      # 100 k-blocks
 ])
 def test_conv_forms(cfg):
     run_conv(*cfg)

@@ -1,6 +1,6 @@
-"""The non-default GEMM feeding paths of the conv kernel -- single-CTA tiles only (DIRB200_CTA2=0), im2col TMA instead of the patch-resident form for the 64 -> 64 3x3 convs (DIRB200_PATCH=0), the cp.async
-gather for the 3x3 / strided convs (DIRB200_IM2COL=0) and for every conv (DIRB200_ATMA=0) -- against torch on the
-shapes of tests/cta2_check.py (the defaults, CTA pairs + tiled / im2col TMA, are what test_gpu_conv*.py exercise).
+"""The non-default GEMM feeding paths of the conv kernel -- the cp.async gather for the 3x3 / strided convs
+(DIRB200_IM2COL=0) and for every conv (DIRB200_ATMA=0) -- against torch on the shapes of tests/cta2_check.py (the
+defaults, tiled / im2col TMA, are what test_gpu_conv*.py exercise).
 The switches are read once per process, so each variant runs tests/cta2_check.py in a subprocess."""
 import os
 import subprocess
@@ -12,9 +12,8 @@ pytestmark = pytest.mark.gpu
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 
 
-@pytest.mark.parametrize("env", [{"DIRB200_CTA2": "0"}, {"DIRB200_IM2COL": "0"}, {"DIRB200_ATMA": "0"},
-                                 {"DIRB200_PATCH": "0"}],
-                         ids=["no_cta_pairs", "gather_for_3x3", "cp_async_gather_only", "im2col_for_64x64_3x3"])
+@pytest.mark.parametrize("env", [{"DIRB200_IM2COL": "0"}, {"DIRB200_ATMA": "0"}],
+                         ids=["gather_for_3x3", "cp_async_gather_only"])
 def test_conv_variant_parity(env):
     e = dict(os.environ)
     e.update(env)

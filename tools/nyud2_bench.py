@@ -1,5 +1,5 @@
 """BASELINE config 4 figures (NYUD2-DIR, synthetic 640x480 -> refinement input [32, 128, 240, 320]): the operators of the
-refinement module R (nyud2-dir/models/modules.py:128-174) on one B200 -- the 5x5 128->128 convolution (fprop / dgrad /
+refinement module R (nyud2-dir/models/modules.py:128-174) on one GPU -- the 5x5 128->128 convolution (fprop / dgrad /
 wgrad), the FDS update over the 2.46 M x 128 pixel features, bilinear up-sampling and the per-pixel LDS-weighted loss
 pieces are timed with CUDA events (L2 flushed between repetitions).  One JSON line; not part of bench.py's headline."""
 import json

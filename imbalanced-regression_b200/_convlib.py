@@ -14,4 +14,10 @@ _lib.register({
     "dirb200_conv_wgrad_workspace_bytes": (c_size_t, _I9 + [c_int]),
     "dirb200_conv_wgrad": (c_int, [P, P, P, P, c_size_t] + _I9 + [c_int, c_int, P]),
     "dirb200_conv_plan": (c_int, _I9 + [c_int, c_int, P]),
+    # test aids: the fused BatchNorm epilogues and their consumers
+    "dirb200_conv_fprop_bn_stats": (c_int, [P, P, P] + _I9 + [c_int, P, P, P]),
+    "dirb200_conv_fprop_affine": (c_int, [P, P, P] + _I9 + [P, P, P, c_int, P]),
+    "dirb200_conv_dgrad_bn_moments": (c_int, [P, P, P] + _I9 + [P, P, P, P, P, P]),
+    "dirb200_bn_finalize_layout": (c_int, [P, P, c_int64, c_int, P, P, c_float, c_float, P, P, P, P, P, P, P]),
+    "dirb200_bn_bwd_coeffs_layout": (c_int, [P, P, c_int64, c_int, P, P, P, P, P, P, P]),
 })

@@ -309,6 +309,51 @@ int dirb200_conv_wgrad(const void* x, const void* dy, float* dw, void* workspace
                     accumulate != 0, as_stream(stream));
 }
 
+/* ---- Test aids: the fused epilogues the network runner uses, one call each (see include/dirb200.h). */
+static void layout_to_host(const StatLayout& l, int* layout_host) {
+  layout_host[0] = l.rows; layout_host[1] = l.n_tiles; layout_host[2] = l.bn; layout_host[3] = l.group;
+}
+
+int dirb200_conv_fprop_bn_stats(const void* x, const void* w_fprop, void* y, int n, int h, int w, int cin, int cout,
+                                int kh, int kw, int stride, int pad, int stem, float* partial, int* layout_host,
+                                void* stream) {
+  DIRB_CHECK_ARG(x && w_fprop && y && partial && layout_host, "conv_fprop_bn_stats: null pointer");
+  ConvShape s;
+  if (int rc = to_shape(n, h, w, cin, cout, kh, kw, stride, pad, stem, &s)) return rc;
+  StatLayout lay{};
+  if (int rc = conv_fprop((const __nv_bfloat16*)x, (const __nv_bfloat16*)w_fprop, (__nv_bfloat16*)y, s, stem != 0,
+                          as_stream(stream), partial, &lay))
+    return rc;
+  layout_to_host(lay, layout_host);
+  return DIRB200_OK;
+}
+
+int dirb200_conv_fprop_affine(const void* x, const void* w_fprop, void* out, int n, int h, int w, int cin, int cout,
+                              int kh, int kw, int stride, int pad, const float* scale, const float* shift,
+                              const void* residual, int relu, void* stream) {
+  DIRB_CHECK_ARG(x && w_fprop && out, "conv_fprop_affine: null pointer");
+  ConvShape s;
+  if (int rc = to_shape(n, h, w, cin, cout, kh, kw, stride, pad, 0, &s)) return rc;
+  return conv_fprop_affine((const __nv_bfloat16*)x, (const __nv_bfloat16*)w_fprop, (__nv_bfloat16*)out, s,
+                           ConvEpilogue{scale, shift, (const __nv_bfloat16*)residual, relu != 0}, as_stream(stream));
+}
+
+int dirb200_conv_dgrad_bn_moments(const void* dy, const void* w_dgrad, void* dx, int n, int h, int w, int cin, int cout,
+                                  int kh, int kw, int stride, int pad, const void* y_prev, const float* scale,
+                                  const float* shift, float* partial, int* layout_host, void* stream) {
+  DIRB_CHECK_ARG(dy && w_dgrad && dx && y_prev && scale && shift && partial && layout_host,
+                 "conv_dgrad_bn_moments: null pointer");
+  ConvShape s;
+  if (int rc = to_shape(n, h, w, cin, cout, kh, kw, stride, pad, 0, &s)) return rc;
+  StatLayout lay{};
+  const DgradBnMoments bm{(const __nv_bfloat16*)y_prev, scale, shift, partial, &lay};
+  if (int rc = conv_dgrad((const __nv_bfloat16*)dy, (const __nv_bfloat16*)w_dgrad, (__nv_bfloat16*)dx, s,
+                          as_stream(stream), &bm))
+    return rc;
+  layout_to_host(lay, layout_host);
+  return DIRB200_OK;
+}
+
 /* Host-only (no CUDA call): the GEMM form dirb200_conv_fprop / _dgrad / _wgrad (op 0 / 1 / 2) would launch for this
  * shape: plan7[0] tile width BN, [1] 0 (no CTA pairs), [2] A-operand form (0 cp.async gather, 1 tiled TMA, 2 im2col
  * TMA), [3] 0 (no patch-resident form), [4] split-K factor, [5] launches, [6] dgrad can carry the BN-backward moments of

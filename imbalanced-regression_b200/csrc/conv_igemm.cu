@@ -165,7 +165,8 @@ igemm_kernel(const __grid_constant__ CUtensorMap tmap_b, const __grid_constant__
   using C = Cfg<BN, !WGRAD>;
   static_assert(BN == 64 || BN == 128, "tile width: one m64n64 / m64n128 wgmma per warpgroup and k step");
   static_assert(!ATMA || !STEM, "TMA-fed A operand: not for the stem");
-  static_assert(!AFFINE || (ATMA && !WGRAD), "folded-BN epilogue: TMA-fed fprop GEMMs only");
+  // the folded-BN epilogue reads only the accumulators and P: it does not depend on how the A operand arrived
+  static_assert(!AFFINE || (!WGRAD && !STEM), "folded-BN epilogue: non-stem fprop GEMMs only");
   static_assert(!BSTAT || (ATMA && !WGRAD && !AFFINE), "BN-backward moments in the epilogue: TMA-fed dgrad GEMMs only");
   extern __shared__ uint8_t smem_raw[];
   const uint32_t smem_base = (smem_u32(smem_raw) + 1023u) & ~1023u;
@@ -772,7 +773,10 @@ static int launch_igemm_impl(const CUtensorMap& tm, const CUtensorMap& tma, cons
                                    cudaFuncAttributeMaxDynamicSharedMemorySize, C::kSmemBytes));
     configured = true;
   }
-  const int grid = Q.num_tiles < num_sms() ? Q.num_tiles : num_sms();
+  int grid = Q.num_tiles < num_sms() ? Q.num_tiles : num_sms();
+  // fprop / dgrad CTAs each keep one n_tile: at least one CTA per n_tile, also when DIRB200_SMS caps the SM count
+  // below the tile count (the extra CTAs run as a second wave)
+  if (!WGRAD && grid < Q.n_tiles) grid = Q.n_tiles;
   t_last_layout = StatLayout{grid, Q.n_tiles, BN, 1};
   igemm_kernel<BN, WGRAD, STEM, ATMA, AFFINE, BSTAT><<<grid, kThreads, C::kSmemBytes, st>>>(tm, tma, Q);
   DIRB_LAUNCHED();
@@ -795,8 +799,12 @@ static int launch_igemm(const CUtensorMap& tm, const IgemmParams& P, int m_tiles
       return launch_igemm_impl<BN, WGRAD, false, true>(tm, *tma, Q, st);
     }
   }
+  if constexpr (!WGRAD && !STEM) {
+    // gather-fed fprop (DIRB200_ATMA=0 / DIRB200_IM2COL=0): the folded-BN epilogue works the same way
+    if (Q.epi_scale != nullptr) return launch_igemm_impl<BN, false, false, false, true>(tm, tm, Q, st);
+  }
   if (Q.epi_scale != nullptr || Q.bst_y != nullptr) {
-    set_error("conv: the folded-BN / BN-backward epilogues need a TMA-fed A operand (DIRB200_ATMA / DIRB200_IM2COL on)");
+    set_error("conv: the BN-backward moments epilogue needs a TMA-fed A operand; the folded-BN one a non-stem fprop");
     return DIRB200_ERR_ARG;
   }
   return launch_igemm_impl<BN, WGRAD, STEM>(tm, tm, Q, st);

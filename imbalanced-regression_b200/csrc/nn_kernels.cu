@@ -945,7 +945,11 @@ static inline int stream_grid(int64_t rows, int lanes) {
   return (int)(g < 1 ? 1 : (g > cap ? cap : g));
 }
 
-int bn_partial_floats(int max_c) { return kReduceCtasPerSm * num_sms() * 3 * max_c; }
+// also holds the [CTA][2][c] rows of a conv epilogue: max(SMs, c / 64) CTAs
+int bn_partial_floats(int max_c) {
+  const int rows = kReduceCtasPerSm * num_sms() * 3, conv_rows = 2 * (max_c / 64);
+  return (rows > conv_rows ? rows : conv_rows) * max_c;
+}
 
 static inline int reduce_grid(int64_t rows, int lanes, int ctas_per_sm = kReduceCtasPerSm) {
   int64_t g = (rows + (int64_t)lanes * 16 - 1) / ((int64_t)lanes * 16);   // >= ~16 rows per thread
@@ -1212,6 +1216,29 @@ int dirb200_bn_train_bwd(const void* grad_out, const void* y, int64_t rows, int 
     return rc;
   return bn_bwd_apply(static_cast<const __nv_bfloat16*>(grad_out), nullptr, static_cast<const __nv_bfloat16*>(y), coef,
                       nullptr, nullptr, sc, sh, nullptr, rows, c, static_cast<__nv_bfloat16*>(grad_y), nullptr, nullptr, st);
+}
+
+/* ---- Test aids: the consumers of the per-CTA rows the conv epilogues write (see include/dirb200.h). */
+int dirb200_bn_finalize_layout(const float* partial, const int* layout_host, int64_t rows, int c, const float* gamma,
+                               const float* beta, float eps, float momentum, float* running_mean, float* running_var,
+                               float* mean_out, float* invstd_out, float* scale_out, float* shift_out, void* stream) {
+  DIRB_CHECK_ARG(partial && layout_host && gamma && beta && mean_out && invstd_out && scale_out && shift_out && rows > 0 &&
+                     c > 0 && (running_mean == nullptr) == (running_var == nullptr),
+                 "bn_finalize_layout: null pointer or bad size");
+  const StatLayout lay{layout_host[0], layout_host[1], layout_host[2], layout_host[3]};
+  return bn_finalize(partial, lay, rows, c, gamma, beta, eps, momentum, running_mean, running_var, mean_out, invstd_out,
+                     scale_out, shift_out, as_stream(stream));
+}
+
+int dirb200_bn_bwd_coeffs_layout(const float* partial, const int* layout_host, int64_t rows, int c, const float* mean,
+                                 const float* invstd, const float* gamma, float* grad_gamma, float* grad_beta,
+                                 float* coef_out, void* stream) {
+  DIRB_CHECK_ARG(partial && layout_host && mean && invstd && gamma && grad_gamma && grad_beta && coef_out && rows > 0 &&
+                     c > 0,
+                 "bn_bwd_coeffs_layout: null pointer or bad size");
+  const StatLayout lay{layout_host[0], layout_host[1], layout_host[2], layout_host[3]};
+  return bn_bwd_coeffs_layout(partial, lay, rows, c, mean, invstd, gamma, grad_gamma, grad_beta, coef_out,
+                              as_stream(stream));
 }
 
 int dirb200_maxpool3x3s2_fwd(const void* x, int n, int h, int w, int c, void* out, uint8_t* argmax, void* stream) {

@@ -272,6 +272,41 @@ int dirb200_conv_wgrad(const void* x, const void* dy, float* dw, void* workspace
                        int n, int h, int w, int cin, int cout, int kh, int kw, int stride, int pad,
                        int stem, int accumulate, void* stream);
 
+/* ------------------------------------------------ Test aids: fused conv epilogues ---- */
+/* The network runner fuses BatchNorm work into the conv epilogues; these entry points run one such launch alone so
+ * that it can be checked against a high-precision reference.  A statistics row layout crosses the ABI as a host
+ * int[4] {rows, n_tiles, bn, group}: channel ch is held in rows (j + k*n_tiles)*group + r, j = ch / bn, k = 0, 1, ..
+ * while the row index < rows, r < group.  Every row the layout names for a channel is written, nothing else.
+ * partial: fp32 [rows][2][C], at most (max(SMs, C / 64) x 2 x C) floats, C = cout (fprop) or cin (dgrad); rows is
+ * min(tiles, SMs), raised to the C / bn column tiles where the SM count is capped below that (DIRB200_SMS). */
+
+/* dirb200_conv_fprop that also writes the per-channel sum (slot 0) and sum of squares (slot 1) of the stored bf16 y. */
+int dirb200_conv_fprop_bn_stats(const void* x, const void* w_fprop, void* y, int n, int h, int w, int cin, int cout,
+                                int kh, int kw, int stride, int pad, int stem, float* partial, int* layout_host,
+                                void* stream);
+/* Inference form (BatchNorm folded into the conv): out = [relu](conv(x, w) * scale[co] + shift[co]) without a
+ * residual; with one (NULL: none; [pixels][cout] bf16) out = [relu](bf16(conv * scale + shift) + residual). */
+int dirb200_conv_fprop_affine(const void* x, const void* w_fprop, void* out, int n, int h, int w, int cin, int cout,
+                              int kh, int kw, int stride, int pad, const float* scale, const float* shift,
+                              const void* residual, int relu, void* stream);
+/* dirb200_conv_dgrad (stride 1; dirb200_conv_plan's plan7[6] says where it applies) that also writes the backward
+ * moments of the BatchNorm + ReLU before it: dz = dx_stored * [y_prev * scale + shift > 0], slot 0 = sum dz,
+ * slot 1 = sum dz * y_prev.  y_prev: [pixels][cin] bf16 like dx. */
+int dirb200_conv_dgrad_bn_moments(const void* dy, const void* w_dgrad, void* dx, int n, int h, int w, int cin, int cout,
+                                  int kh, int kw, int stride, int pad, const void* y_prev, const float* scale,
+                                  const float* shift, float* partial, int* layout_host, void* stream);
+/* BatchNorm batch statistics from the rows of dirb200_conv_fprop_bn_stats (rows = pixels): mean, invstd (biased
+ * variance), scale = gamma * invstd, shift = beta - mean * scale; running statistics (NULL: not tracked) updated with
+ * `momentum` and the unbiased variance. */
+int dirb200_bn_finalize_layout(const float* partial, const int* layout_host, int64_t rows, int c, const float* gamma,
+                               const float* beta, float eps, float momentum, float* running_mean, float* running_var,
+                               float* mean_out, float* invstd_out, float* scale_out, float* shift_out, void* stream);
+/* BatchNorm backward coefficients from the rows of dirb200_conv_dgrad_bn_moments: dgamma = invstd * (S1 - mean * S0),
+ * dbeta = S0 (both ACCUMULATED into grad_gamma / grad_beta); coef_out [3][c] = A, B, C of dy = A*dz + B*y + C. */
+int dirb200_bn_bwd_coeffs_layout(const float* partial, const int* layout_host, int64_t rows, int c, const float* mean,
+                                 const float* invstd, const float* gamma, float* grad_gamma, float* grad_beta,
+                                 float* coef_out, void* stream);
+
 /* ------------------------------------------------ ResNet backbone runner ---- */
 /* Opaque native runner of the bottleneck ResNet of agedb-dir/resnet.py:41-70,
  * 73-138 (conv1/bn1/relu/maxpool, layer1-4, avgpool, view) for one fixed

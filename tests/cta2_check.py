@@ -1,7 +1,8 @@
 """Standalone GPU check + per-layer timing of the conv GEMMs under the kernel's run-time switches (not collected
 by pytest; tests/test_gpu_conv_variants.py runs the parity half in subprocesses).
 
-    python tests/cta2_check.py parity                    # defaults: tiled / im2col TMA
+    python tests/cta2_check.py parity                    # defaults: tiled / im2col TMA (plain GEMMs + fused
+                                                          # BN-statistics and folded-BN epilogues)
     DIRB200_IM2COL=0 python tests/cta2_check.py parity   # cp.async gather for the 3x3 / strided convs
     DIRB200_ATMA=0   python tests/cta2_check.py parity   # cp.async gather for every conv
     <switches> python tests/cta2_check.py time [substr]  # per-layer fprop/dgrad/wgrad times, batch-256 ResNet-50 shapes
@@ -72,22 +73,28 @@ LAYERS = [
 
 def parity():
     from test_gpu_conv import run_conv
+    import test_gpu_conv_epilogues as E
+    # the plain GEMMs, then the fused BatchNorm epilogues (statistics + finalize, folded BN) of
+    # tests/test_gpu_conv_epilogues.py on its shapes
+    cases = [(run_conv, cfg) for cfg in PARITY]
+    cases += [(E.test_fprop_bn_stats_and_finalize, s) for s in E.SHAPES]
+    cases += [(E.test_fprop_affine_epilogue, s) for s in E.SHAPES]
     bad = 0
-    for cfg in PARITY:
+    for fn, cfg in cases:
         try:
-            run_conv(*cfg)
+            fn(*cfg) if fn is run_conv else fn(cfg)
             torch.cuda.synchronize()
-            print("PASS", cfg, flush=True)
+            print("PASS", fn.__name__, cfg, flush=True)
         except Exception as e:  # noqa: BLE001
             bad += 1
-            print("FAIL", cfg, repr(e)[:300], flush=True)
+            print("FAIL", fn.__name__, cfg, repr(e)[:300], flush=True)
             traceback.print_exc()
             try:
                 torch.cuda.synchronize()
             except Exception:  # noqa: BLE001  (sticky CUDA error: nothing more can run in this process)
                 print("CUDA context lost; stopping", flush=True)
                 break
-    print(f"parity: {len(PARITY) - bad}/{len(PARITY)} ok (switches: " + " ".join(f"{k}={v}" for k, v in os.environ.items() if k.startswith("DIRB200_")) + ")")
+    print(f"parity: {len(cases) - bad}/{len(cases)} ok (switches: " + " ".join(f"{k}={v}" for k, v in os.environ.items() if k.startswith("DIRB200_")) + ")")
     return bad
 
 

@@ -126,3 +126,45 @@ def test_conv_plan_selects_the_intended_gemm_forms():
     # 5x5 (NYUD2 refinement conv) goes through im2col TMA as well; the stem keeps the cp.async gather
     assert plan(240, 128, 128, 5, 1, 2, 0)["feed"] == IM2COL
     assert plan(224, 3, 64, 7, 2, 3, 0, stem=1)["feed"] == GATHER
+
+
+def test_fused_epilogue_test_aids_refuse_bad_arguments_before_any_cuda_call():
+    """The test-aid entry points of the fused conv epilogues validate their arguments on the host: each call below
+    is refused with rc -1 and a message, without a device (every pointer is a dummy that must never be dereferenced)."""
+    import ctypes
+    import _lib, _convlib  # noqa: F401
+    d = ctypes.c_void_p(16)                   # stands for a device buffer
+    lay = (ctypes.c_int * 4)(128, 1, 64, 1)
+
+    def refused(name, *args, msg):
+        rc = _lib.raw(name)(*args)
+        err = _lib.last_error()
+        assert rc == -1 and msg in err, (name, rc, err)
+
+    s1 = (2, 8, 8, 64, 64, 3, 3, 1, 1)       # n, h, w, cin, cout, kh, kw, stride, pad
+    s2 = (2, 8, 8, 64, 64, 3, 3, 2, 1)
+    # BN-backward moments on a stride-2 dgrad (its parity-class launches have no fused form)
+    refused("dirb200_conv_dgrad_bn_moments", d, d, d, *s2, d, d, d, d, lay, None, msg="stride-1")
+    # the folded-BN epilogue without its scale or shift
+    refused("dirb200_conv_fprop_affine", d, d, d, *s1, None, d, None, 1, None, msg="scale / shift")
+    refused("dirb200_conv_fprop_affine", d, d, d, *s1, d, None, d, 0, None, msg="scale / shift")
+    # Cout not a multiple of 64
+    bad_cout = (2, 8, 8, 64, 96, 1, 1, 1, 0)
+    refused("dirb200_conv_fprop_bn_stats", d, d, d, *bad_cout, 0, d, lay, None, msg="multiple of 64")
+    refused("dirb200_conv_fprop_affine", d, d, d, *bad_cout, d, d, None, 1, None, msg="multiple of 64")
+    refused("dirb200_conv_dgrad_bn_moments", d, d, d, *(2, 8, 8, 96, 64, 1, 1, 1, 0), d, d, d, d, lay, None,
+            msg="multiple of 64")
+    # null pointers
+    refused("dirb200_conv_fprop_bn_stats", d, d, d, *s1, 0, None, lay, None, msg="null")
+    refused("dirb200_conv_fprop_bn_stats", d, d, d, *s1, 0, d, None, None, msg="null")
+    refused("dirb200_conv_fprop_affine", None, d, d, *s1, d, d, None, 1, None, msg="null")
+    refused("dirb200_conv_dgrad_bn_moments", d, d, d, *s1, None, d, d, d, lay, None, msg="null")
+    refused("dirb200_conv_dgrad_bn_moments", d, d, d, *s1, d, d, d, None, lay, None, msg="null")
+    refused("dirb200_bn_finalize_layout", None, lay, 128, 64, d, d, 1e-5, 0.1, d, d, d, d, d, d, None, msg="null")
+    refused("dirb200_bn_finalize_layout", d, None, 128, 64, d, d, 1e-5, 0.1, d, d, d, d, d, d, None, msg="null")
+    refused("dirb200_bn_bwd_coeffs_layout", d, lay, 128, 64, d, d, d, None, d, d, None, msg="null")
+    # a layout whose tiles do not cover the channels
+    short = (ctypes.c_int * 4)(128, 1, 32, 1)
+    refused("dirb200_bn_finalize_layout", d, short, 128, 64, d, d, 1e-5, 0.1, None, None, d, d, d, d, None,
+            msg="layout")
+    refused("dirb200_bn_bwd_coeffs_layout", d, short, 128, 64, d, d, d, d, d, d, None, msg="layout")

@@ -264,6 +264,10 @@ def test_eval_forward_folded_bn_layerwise_vs_oracle(n, hw):
         e = rel(got, ref)
         assert e <= tol, (name, e)
 
+    # DIRB200_FOLDED_EVAL=0: conv -> bf16 raw output -> separate BN-apply pass, so the buffers hold other stages:
+    # peek(b, 5) is the RAW downsample output, and the block tail adds the two BN outputs in fp32 before one rounding
+    folded = os.environ.get("DIRB200_FOLDED_EVAL", "1")[:1] != "0"
+    stored = (lambda t: t) if folded else q     # the unfused path stores the conv output in bf16 before the BN
     with torch.no_grad():
         sc, sh = fold("bn1.")
         check("stem.pool", pk(-1, 6), F.max_pool2d(q(F.relu(pk(-1, 0) * sc + sh)), 3, 2, 1))
@@ -274,18 +278,28 @@ def test_eval_forward_folded_bn_layerwise_vs_oracle(n, hw):
                 pre = f"layer{li + 1}.{b}."
                 xin = pk(-1, 6) if bi == 0 else pk(bi - 1, 6)
                 sc, sh = fold(pre + "bn1.")
-                check(pre + "conv1+bn1", pk(bi, 1), q(F.relu(conv(xin, sd[pre + "conv1.weight"], 1, 0) * sc + sh)))
+                check(pre + "conv1+bn1", pk(bi, 1), q(F.relu(stored(conv(xin, sd[pre + "conv1.weight"], 1, 0)) * sc + sh)))
                 sc, sh = fold(pre + "bn2.")
-                check(pre + "conv2+bn2", pk(bi, 3), q(F.relu(conv(pk(bi, 1), sd[pre + "conv2.weight"], stride, 1) * sc + sh)))
+                check(pre + "conv2+bn2", pk(bi, 3),
+                      q(F.relu(stored(conv(pk(bi, 1), sd[pre + "conv2.weight"], stride, 1)) * sc + sh)))
                 if pre + "downsample.0.weight" in sd:
                     sc, sh = fold(pre + "downsample.1.")
-                    check(pre + "ds", pk(bi, 5), q(conv(xin, sd[pre + "downsample.0.weight"], stride, 0) * sc + sh))
-                    idn = pk(bi, 5)
+                    if folded:
+                        check(pre + "ds", pk(bi, 5), q(conv(xin, sd[pre + "downsample.0.weight"], stride, 0) * sc + sh))
+                        idn = pk(bi, 5)
+                    else:
+                        check(pre + "ds raw", pk(bi, 5), q(conv(xin, sd[pre + "downsample.0.weight"], stride, 0)))
+                        idn = pk(bi, 5) * sc + sh
                 else:
                     idn = xin
                 sc, sh = fold(pre + "bn3.")
-                # the epilogue rounds the BN output to bf16 before the shortcut is added (staging tile), then rounds again
-                check(pre + "out", pk(bi, 6), q(F.relu(q(conv(pk(bi, 3), sd[pre + "conv3.weight"], 1, 0) * sc + sh) + idn)))
+                y3 = conv(pk(bi, 3), sd[pre + "conv3.weight"], 1, 0)
+                if folded:
+                    # the epilogue rounds the BN output to bf16 before the shortcut is added (staging tile), then
+                    # rounds again
+                    check(pre + "out", pk(bi, 6), q(F.relu(q(y3 * sc + sh) + idn)))
+                else:
+                    check(pre + "out", pk(bi, 6), q(F.relu(q(y3) * sc + sh + idn)))
                 bi += 1
         # end to end: torch's own eval-mode network on the same parameters and running statistics (fp32)
         def bn(t, pre):

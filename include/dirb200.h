@@ -227,6 +227,23 @@ int dirb200_int_label_histogram(const float* labels, int64_t n, int nbins, int64
 int dirb200_shot_metrics(const float* preds, const float* labels, int64_t n, const int64_t* train_hist, int nbins,
                          int many_shot_thr, int low_shot_thr, double* out16, void* stream);
 
+/* NYUD2-DIR depth evaluation in one fused pass (replaces nyud2-dir/test.py:52-55 -- F.interpolate(align_corners=True),
+ * output[mask], the per-image .cpu() -- and Evaluator.__call__ / evaluate / evaluate_shot, nyud2-dir/util.py:35-133).
+ * pred fp32 [n_images][ph][pw]; target fp32 and mask u8 [n_images][h][w] (mask NULL: every pixel).  When
+ * (ph, pw) != (h, w) the prediction is ATen's CUDA upsample_bilinear2d with align_corners = True, formed in registers
+ * for the masked pixels only; equal sizes copy.  Per-pixel terms in fp32 as Evaluator.evaluate forms them (a NaN
+ * target zeroes them), widened to fp64 and summed.  Shot group of a finite target: bin = min(int(t * 10.f), 99)
+ * (fp32 product, truncation toward zero), group_of_bin[bin] for 0 <= bin < nbins (u8: 0 none, 1 many, 2 medium,
+ * 3 few; NULL iff nbins == 0); NaN / inf targets belong to no group.
+ * acc double[4][10], ADDED to (stream an evaluation batch by batch): rows overall, many, medium, few; columns NUM
+ * (non-NaN targets), sum d^2, sum d, sum d/t, sum |lg10 o - lg10 t|, delta1-3 counts (max(o/t, t/o) <= 1.25^k),
+ * NaN-target count, +-inf-target count (d = |o - t|).  Deterministic: per-CTA partials in `workspace`, summed in
+ * CTA order by the last CTA; one kernel launch. */
+size_t dirb200_depth_metrics_workspace_bytes(int64_t n_images, int h, int w);
+int dirb200_depth_metrics_accumulate(const float* pred, int ph, int pw, const float* target, const uint8_t* mask,
+                                     int64_t n_images, int h, int w, const uint8_t* group_of_bin, int nbins,
+                                     double* acc, void* workspace, size_t workspace_bytes, void* stream);
+
 /* ------------------------------------------------- convolution stack ---- */
 /* Activations are NHWC bf16; weights arrive in the reference's fp32
  * [Cout][Cin][KH][KW] layout (agedb-dir/resnet.py:46-51,79,112-118, i.e. the

@@ -30,9 +30,11 @@ int bn_apply(const __nv_bfloat16* y, const float* scale, const float* shift, con
 // g2_h, g2_w > 0: g2 is the COMPACT [n, g2_h/2, g2_w/2, c] gradient of a stride-2 1x1 downsample conv (added at even y, x)
 // dz_out (identity blocks): dz = (g1 [+ g2]) * mask is stored and summed as stored; bn_bwd_apply then takes dz as its
 // only gradient input (mask == scale == shift == nullptr)
+// g3 (with g2 and dz_out only): a third dense gradient, summed in fp32 with g1 + g2 before dz is rounded to bf16
 int bn_bwd_reduce(const __nv_bfloat16* g1, const __nv_bfloat16* g2, const __nv_bfloat16* y, const __nv_bfloat16* y2,
                   const float* scale, const float* shift, const uint8_t* mask, int64_t rows, int c, float* partial,
-                  int* nblocks, cudaStream_t st, int g2_h = 0, int g2_w = 0, __nv_bfloat16* dz_out = nullptr);
+                  int* nblocks, cudaStream_t st, int g2_h = 0, int g2_w = 0, __nv_bfloat16* dz_out = nullptr,
+                  const __nv_bfloat16* g3 = nullptr);
 int bn_bwd_coeffs(const float* partial, int nblocks, int k, int gslot, int64_t rows, int c, const float* mean,
                   const float* invstd, const float* gamma, float* grad_gamma, float* grad_beta, float* coef,
                   cudaStream_t st);

@@ -356,10 +356,13 @@ struct CompactG2 {
 
 // WRITE_DZ (identity blocks): dz is stored (bf16) -- it is the gradient of the shortcut path anyway -- and the sums
 // are taken over the STORED values, so that bn_bwd_apply can read dz (one tensor) instead of g1, g2 and the mask again.
-template <int MODE, int G2M, bool HAS_Y2, bool WRITE_DZ>
+// HAS_G3 (identity blocks whose output is also a block output of the multi-scale encoder): a third dense gradient g3,
+// added in fp32 to g1 + g2 before the mask and the one bf16 rounding of dz.
+template <int MODE, int G2M, bool HAS_Y2, bool WRITE_DZ, bool HAS_G3 = false>
 __global__ void __launch_bounds__(256, 3)
 bn_bwd_reduce_kernel(const __nv_bfloat16* __restrict__ g1, const __nv_bfloat16* __restrict__ g2, CompactG2 cg2,
-                     const __nv_bfloat16* __restrict__ y, const __nv_bfloat16* __restrict__ y2,
+                     const __nv_bfloat16* __restrict__ g3, const __nv_bfloat16* __restrict__ y,
+                     const __nv_bfloat16* __restrict__ y2,
                      const float* __restrict__ scale, const float* __restrict__ shift,
                      const uint8_t* __restrict__ mask, int64_t rows, int c, float* __restrict__ partial,
                      __nv_bfloat16* __restrict__ dz_out) {
@@ -376,10 +379,14 @@ bn_bwd_reduce_kernel(const __nv_bfloat16* __restrict__ g1, const __nv_bfloat16* 
     const int64_t r1 = r0 + stride;
     const bool two = r1 < rows;
     const int64_t o0 = r0 * c + cg * 8, o1 = (two ? r1 : r0) * c + cg * 8;
-    uint4 G[2], Y[2], G2[2], Y2[2];
+    uint4 G[2], Y[2], G2[2], Y2[2], G3[2];
     uint32_t M[2];
     G[0] = *reinterpret_cast<const uint4*>(g1 + o0);
     G[1] = *reinterpret_cast<const uint4*>(g1 + o1);
+    if (HAS_G3) {
+      G3[0] = *reinterpret_cast<const uint4*>(g3 + o0);
+      G3[1] = *reinterpret_cast<const uint4*>(g3 + o1);
+    }
     Y[0] = *reinterpret_cast<const uint4*>(y + o0);
     Y[1] = *reinterpret_cast<const uint4*>(y + o1);
     if (G2M == G2_DENSE) {
@@ -408,6 +415,12 @@ bn_bwd_reduce_kernel(const __nv_bfloat16* __restrict__ g1, const __nv_bfloat16* 
         if (HAS_G2) {
           const uint32_t g2w[4] = {G2[u].x, G2[u].y, G2[u].z, G2[u].w};
           const float2 t = bf2_to_f2(g2w[w]);
+          g.x += t.x;
+          g.y += t.y;
+        }
+        if (HAS_G3) {
+          const uint32_t g3w[4] = {G3[u].x, G3[u].y, G3[u].z, G3[u].w};
+          const float2 t = bf2_to_f2(g3w[w]);
           g.x += t.x;
           g.y += t.y;
         }
@@ -1048,8 +1061,9 @@ static CompactG2 make_compact(int g2_h, int g2_w) {
 // g2_h, g2_w > 0: g2 is the compact [n, g2_h/2, g2_w/2, c] tensor (rows are the pixels of the g2_h x g2_w maps)
 int bn_bwd_reduce(const __nv_bfloat16* g1, const __nv_bfloat16* g2, const __nv_bfloat16* y, const __nv_bfloat16* y2,
                   const float* scale, const float* shift, const uint8_t* mask, int64_t rows, int c, float* partial,
-                  int* nblocks, cudaStream_t st, int g2_h, int g2_w, __nv_bfloat16* dz_out) {
+                  int* nblocks, cudaStream_t st, int g2_h, int g2_w, __nv_bfloat16* dz_out, const __nv_bfloat16* g3) {
   const CompactG2 cg2 = make_compact(g2_h, g2_w);
+  DIRB_CHECK_ARG(!g3 || (g2 && dz_out), "bn_bwd_reduce: a third gradient is added in the two-gradient identity forms only");
   DIRB_CHECK_ARG(g2_h == 0 || (g2 && mask && !y2 && g2_h % 2 == 0 && g2_w % 2 == 0 && rows % ((int64_t)g2_h * g2_w) == 0),
                  "bn_bwd_reduce: bad compact second gradient");
   const int cgroups = c / 8;
@@ -1059,14 +1073,17 @@ int bn_bwd_reduce(const __nv_bfloat16* g1, const __nv_bfloat16* g2, const __nv_b
   DIRB_CHECK_ARG(!dz_out || (mask && !y2), "bn_bwd_reduce: dz is stored for identity blocks only");
   const int lanes = 256 / cgroups;
   const size_t smem = 256 * (y2 ? 24 : 16) * sizeof(float);
-#define DIRB_RED(MODE, G2, Y2, DZ)                                                                            \
-  do {                                                                                                        \
-    static const int occ = resident_ctas(bn_bwd_reduce_kernel<MODE, G2, Y2, DZ>, 256 * 24 * sizeof(float));   \
-    *nblocks = reduce_grid(rows, lanes, occ);                                                                 \
-    bn_bwd_reduce_kernel<MODE, G2, Y2, DZ><<<*nblocks, 256, smem, st>>>(g1, g2, cg2, y, y2, scale, shift, mask, rows, c, \
-                                                                        partial, dz_out);                     \
+#define DIRB_RED3(MODE, G2, Y2, DZ, G3)                                                                             \
+  do {                                                                                                              \
+    static const int occ = resident_ctas(bn_bwd_reduce_kernel<MODE, G2, Y2, DZ, G3>, 256 * 24 * sizeof(float));     \
+    *nblocks = reduce_grid(rows, lanes, occ);                                                                       \
+    bn_bwd_reduce_kernel<MODE, G2, Y2, DZ, G3><<<*nblocks, 256, smem, st>>>(g1, g2, cg2, g3, y, y2, scale, shift, mask, \
+                                                                            rows, c, partial, dz_out);              \
   } while (0)
-  if (!mask && !scale) DIRB_RED(MASK_NONE, G2_NONE, false, false);        // BN without a ReLU behind it
+#define DIRB_RED(MODE, G2, Y2, DZ) DIRB_RED3(MODE, G2, Y2, DZ, false)
+  if (g3 && g2_h) DIRB_RED3(MASK_BITS, G2_COMPACT, false, true, true);
+  else if (g3) DIRB_RED3(MASK_BITS, G2_DENSE, false, true, true);
+  else if (!mask && !scale) DIRB_RED(MASK_NONE, G2_NONE, false, false);   // BN without a ReLU behind it
   else if (!mask) DIRB_RED(MASK_FROM_Y, G2_NONE, false, false);
   else if (g2_h && dz_out) DIRB_RED(MASK_BITS, G2_COMPACT, false, true);
   else if (g2_h) DIRB_RED(MASK_BITS, G2_COMPACT, false, false);
@@ -1077,6 +1094,7 @@ int bn_bwd_reduce(const __nv_bfloat16* g1, const __nv_bfloat16* g2, const __nv_b
   else if (dz_out) DIRB_RED(MASK_BITS, G2_NONE, false, true);
   else DIRB_RED(MASK_BITS, G2_NONE, false, false);
 #undef DIRB_RED
+#undef DIRB_RED3
   DIRB_LAUNCHED();
   return DIRB200_OK;
 }

@@ -83,6 +83,12 @@ struct dirb200_net {
     int gB_h = 0, gB_w = 0;
   };
   GraphSlot g_fwd, g_bwd[6];
+  // multi-scale (encoder) mode, dirb200_resnet_forward_blocks / dirb200_resnet_backward_blocks_stage: graphs of their
+  // own.  A backward stage's sequence depends on the topmost stage that received a gradient (it fixes which scratch
+  // buffers hold the incoming pair) and on whether the stage's own block gradient is added: [stage][top][d_block]
+  GraphSlot g_fwd_blocks, g_bwd_blocks[6][6][2];
+  bool bwd_blocks = false;   // the pending backward is the multi-scale one
+  int bwd_top = -1;          // multi-scale backward: topmost stage that received a gradient so far (-1: none)
   cudaStream_t cap_stream = nullptr;               // capture happens on a private stream (the caller's may be the legacy default stream, which cannot capture)
   float *enc_buf = nullptr, *denc_buf = nullptr;   // fixed-address copies of the forward's output / the backward's input
   // optional per-kernel-class timing (CUDA events around every launch group)
@@ -361,6 +367,7 @@ static bool folded_eval() {
   return on;
 }
 
+// enc_out == nullptr: no average pool (multi-scale mode reads the block outputs)
 static int forward_eval_folded(dirb200_net* net, const float* params, const float* running, float* enc_out,
                                cudaStream_t st) {
   RUNP(kBnStats, bn_eval_coeffs_all(net->bn_eval_descs, net->num_bns, net->max_bn_c, params, running, 1e-5f, st));
@@ -378,7 +385,42 @@ static int forward_eval_folded(dirb200_net* net, const float* params, const floa
     }
     RUNP(kFprop, conv_fprop_affine(B.c2.a, B.c3.wf, B.out, B.c3.s, ConvEpilogue{B.c3.bn.scale, B.c3.bn.shift, shortcut, true}, st));
   }
-  RUNP(kPool, avgpool_fwd(net->blocks.back().out, net->n, net->feat_hw, net->feat_c, enc_out, st));
+  if (enc_out) RUNP(kPool, avgpool_fwd(net->blocks.back().out, net->n, net->feat_hw, net->feat_c, enc_out, st));
+  return DIRB200_OK;
+}
+
+// The launch sequence of a forward after the input re-layout (training: batch statistics; else the unfused eval form).
+// enc_out == nullptr: no average pool.
+static int forward_body(dirb200_net* net, const float* params, float* running, bool tr, float* enc_out,
+                        cudaStream_t st) {
+  RUN(conv_bn_forward(net, net->stem, net->x_s2d, params, running, tr, st));       // stem.a == nullptr: no bn_apply
+  RUNP(kPool, bn_relu_maxpool_fwd(net->stem.y, net->stem.bn.scale, net->stem.bn.shift, net->n, net->stem.s.ho,
+                                  net->stem.s.wo, 64, net->pool_out, net->pool_idx, st));
+  for (Block& B : net->blocks) {
+    RUN(conv_bn_forward(net, B.c1, B.in, params, running, tr, st));
+    RUN(conv_bn_forward(net, B.c2, B.c1.a, params, running, tr, st));
+    RUN(conv_bn_forward(net, B.c3, B.c2.a, params, running, tr, st));
+    if (B.has_ds) {
+      RUN(conv_bn_forward(net, B.ds, B.in, params, running, tr, st));
+      RUNP(kBnApply, bn_apply(B.c3.y, B.c3.bn.scale, B.c3.bn.shift, nullptr, B.ds.y, B.ds.bn.scale, B.ds.bn.shift, true,
+                              B.c3.rows, B.c3.bn.c, B.out, tr ? B.mask : nullptr, st));
+    } else {
+      RUNP(kBnApply, bn_apply(B.c3.y, B.c3.bn.scale, B.c3.bn.shift, B.in, nullptr, nullptr, nullptr, true, B.c3.rows,
+                              B.c3.bn.c, B.out, tr ? B.mask : nullptr, st));
+    }
+  }
+  if (enc_out) RUNP(kPool, avgpool_fwd(net->blocks.back().out, net->n, net->feat_hw, net->feat_c, enc_out, st));
+  return DIRB200_OK;
+}
+
+// Multi-scale mode hands out (and takes a gradient for) the output of the last block of every layer group; that block
+// must be an identity block (true of every layer group of ResNet-50 and deeper), whose output BN-backward reduction
+// takes the group's gradient as a third operand.
+static int check_blocks_mode(const dirb200_net* net, const char* who) {
+  const int nst = (int)net->stage_begin.size() - 2;
+  for (int s = 1; s <= nst; ++s)
+    DIRB_CHECK_ARG(!net->blocks[net->stage_begin[s + 1] - 1].has_ds,
+                   "%s: layer group %d ends in a downsample block; multi-scale mode needs an identity block there", who, s);
   return DIRB200_OK;
 }
 
@@ -464,11 +506,25 @@ static int dgrad_with_bn_moments(dirb200_net* net, const __nv_bfloat16* dy, Conv
 
 }  // namespace dirb200
 
+// bounds of the packed pixel coordinates of the convolutions (see dirb200_resnet_create)
+static constexpr int kMaxNetBatch = 1 << 13;        // image index: 13 bits
+static constexpr int kMaxNetSide = 2 * (1 << 9);    // stem-output row / column: 9 bits, the stem halves H and W
+
 extern "C" {
 
 int dirb200_resnet_create(int n, int h, int w, const int* blocks_per_stage, int num_stages, dirb200_net** out) {
   DIRB_CHECK_ARG(out && blocks_per_stage && n > 0 && num_stages >= 1 && num_stages <= 4, "resnet_create: bad arguments");
-  DIRB_CHECK_ARG(h > 0 && w > 0 && h % 32 == 0 && w % 32 == 0, "resnet_create: H and W must be multiples of 32");
+  // the input space-to-depth needs even H and W, the max-pool backward an even stem output (H/2, W/2)
+  DIRB_CHECK_ARG(h > 0 && w > 0 && h % 4 == 0 && w % 4 == 0, "resnet_create: H and W must be multiples of 4 (got %dx%d)",
+                 h, w);
+  // the implicit-GEMM convolutions pack a pixel of the largest map they index (the stem output, H/2 x W/2) as
+  // image (13 bits) | row (9 bits) | column (9 bits) (conv_igemm.cu, pack_pixel / row_pre), and that map must hold
+  // fewer than 2^31 pixels
+  DIRB_CHECK_ARG(n <= kMaxNetBatch, "resnet_create: N must be at most %d (got %d)", kMaxNetBatch, n);
+  DIRB_CHECK_ARG(h <= kMaxNetSide && w <= kMaxNetSide, "resnet_create: H and W must be at most %d (got %dx%d)", kMaxNetSide,
+                 h, w);
+  DIRB_CHECK_ARG((int64_t)n * (h / 2) * (w / 2) < (int64_t(1) << 31),
+                 "resnet_create: N * H/2 * W/2 must be below 2^31 (got %d x %d x %d)", n, h / 2, w / 2);
   dirb200_net* net = new dirb200_net();
   net->n = n; net->h = h; net->w = w;
   if (!build(net, blocks_per_stage, num_stages)) {
@@ -484,8 +540,13 @@ void dirb200_resnet_destroy(dirb200_net* net) {
   if (!net) return;
   if (net->cap_stream) cudaStreamDestroy(net->cap_stream);
   if (net->g_fwd.exec) cudaGraphExecDestroy(net->g_fwd.exec);
+  if (net->g_fwd_blocks.exec) cudaGraphExecDestroy(net->g_fwd_blocks.exec);
   for (auto& g : net->g_bwd)
     if (g.exec) cudaGraphExecDestroy(g.exec);
+  for (auto& per_stage : net->g_bwd_blocks)
+    for (auto& per_top : per_stage)
+      for (auto& g : per_top)
+        if (g.exec) cudaGraphExecDestroy(g.exec);
   for (void* p : net->allocs) cudaFree(p);
   delete net;
 }
@@ -538,26 +599,7 @@ int dirb200_resnet_forward(dirb200_net* net, const float* x_nchw, const float* p
   }
   const bool graphed = tr && graphs_enabled() && !net->profiling;
   float* enc_dst = graphed ? net->enc_buf : enc_out;
-  auto body = [&](cudaStream_t st) -> int {
-    RUN(conv_bn_forward(net, net->stem, net->x_s2d, params, bn_running, tr, st));       // stem.a == nullptr: no bn_apply
-    RUNP(kPool, bn_relu_maxpool_fwd(net->stem.y, net->stem.bn.scale, net->stem.bn.shift, net->n, net->stem.s.ho,
-                                    net->stem.s.wo, 64, net->pool_out, net->pool_idx, st));
-    for (Block& B : net->blocks) {
-      RUN(conv_bn_forward(net, B.c1, B.in, params, bn_running, tr, st));
-      RUN(conv_bn_forward(net, B.c2, B.c1.a, params, bn_running, tr, st));
-      RUN(conv_bn_forward(net, B.c3, B.c2.a, params, bn_running, tr, st));
-      if (B.has_ds) {
-        RUN(conv_bn_forward(net, B.ds, B.in, params, bn_running, tr, st));
-        RUNP(kBnApply, bn_apply(B.c3.y, B.c3.bn.scale, B.c3.bn.shift, nullptr, B.ds.y, B.ds.bn.scale, B.ds.bn.shift, true,
-                                B.c3.rows, B.c3.bn.c, B.out, tr ? B.mask : nullptr, st));
-      } else {
-        RUNP(kBnApply, bn_apply(B.c3.y, B.c3.bn.scale, B.c3.bn.shift, B.in, nullptr, nullptr, nullptr, true, B.c3.rows,
-                                B.c3.bn.c, B.out, tr ? B.mask : nullptr, st));
-      }
-    }
-    RUNP(kPool, avgpool_fwd(net->blocks.back().out, net->n, net->feat_hw, net->feat_c, enc_dst, st));
-    return DIRB200_OK;
-  };
+  auto body = [&](cudaStream_t st) -> int { return forward_body(net, params, bn_running, tr, enc_dst, st); };
   if (graphed) {
     RUN(run_graphed(net, net->g_fwd, params, bn_running, st, body));
     DIRB_CUDA(cudaMemcpyAsync(enc_out, net->enc_buf, sizeof(float) * (size_t)net->n * net->feat_c,
@@ -569,12 +611,45 @@ int dirb200_resnet_forward(dirb200_net* net, const float* x_nchw, const float* p
   return DIRB200_OK;
 }
 
+/* The same forward without the average pool (nyud2-dir/models/modules.py:33-58, E_resnet.forward): the output of the
+ * last block of layer group s+1 goes to block_out[s], NHWC bf16 [n, h_s, w_s, C_s].  training == 0: the folded-BN
+ * inference forward.  The training launch sequence is graph-replayed (a graph of its own) and the outputs are copied
+ * out after it, so the caller's pointers may change from call to call. */
+int dirb200_resnet_forward_blocks(dirb200_net* net, const float* x_nchw, const float* params, float* bn_running,
+                                  int training, void* const* block_out, void* stream) {
+  DIRB_CHECK_ARG(net && x_nchw && params && block_out, "resnet_forward_blocks: null pointer");
+  DIRB_CHECK_ARG(training || bn_running, "resnet_forward_blocks: eval mode needs the running statistics");
+  const int nst = (int)net->stage_begin.size() - 2;
+  for (int s = 0; s < nst; ++s) DIRB_CHECK_ARG(block_out[s], "resnet_forward_blocks: null block_out[%d]", s);
+  RUN(check_blocks_mode(net, "resnet_forward_blocks"));
+  cudaStream_t st = as_stream(stream);
+  const bool tr = training != 0;
+  RUNP(kPrep, prep_weights_all(params, net->prep_descs, net->num_convs, st));
+  RUNP(kPrep, input_to_s2d(x_nchw, net->n, net->h, net->w, net->x_s2d, st));
+  if (!tr && folded_eval()) {
+    RUN(forward_eval_folded(net, params, bn_running, nullptr, st));
+  } else {
+    auto body = [&](cudaStream_t st) -> int { return forward_body(net, params, bn_running, tr, nullptr, st); };
+    if (tr) RUN(run_graphed(net, net->g_fwd_blocks, params, bn_running, st, body));
+    else RUN(body(st));
+  }
+  for (int s = 0; s < nst; ++s) {
+    const Block& B = net->blocks[net->stage_begin[s + 2] - 1];
+    DIRB_CUDA(cudaMemcpyAsync(block_out[s], B.out, sizeof(__nv_bfloat16) * (size_t)B.c3.rows * B.c3.s.cout,
+                              cudaMemcpyDeviceToDevice, st));
+  }
+  net->forward_was_training = tr;
+  return DIRB200_OK;
+}
+
 }  // extern "C"
 
 namespace dirb200 {
 
-// blocks [lo, hi) in reverse order; the incoming gradient pair is net->bw_gA / bw_gB
-static int backward_blocks(dirb200_net* net, int lo, int hi, const float* params, float* grads, cudaStream_t st) {
+// blocks [lo, hi) in reverse order; the incoming gradient pair is net->bw_gA / bw_gB, plus g3 (may be null) for the
+// output of block hi-1 (multi-scale mode: the gradient of a layer group's output from outside the network)
+static int backward_blocks(dirb200_net* net, int lo, int hi, const float* params, float* grads, cudaStream_t st,
+                           const __nv_bfloat16* g3 = nullptr) {
   __nv_bfloat16 *gA = net->bw_gA, *gB = net->bw_gB, *nA = net->bw_nA, *nB = net->bw_nB, *spareB = net->bw_spareB;
   __nv_bfloat16 *t1 = net->scratch[4], *t2 = net->scratch[5], *t3 = net->scratch[6];
   int gB_h = net->bw_gB_h, gB_w = net->bw_gB_w;
@@ -587,7 +662,8 @@ static int backward_blocks(dirb200_net* net, int lo, int hi, const float* params
     // identity blocks: the reduction also stores dz (= the gradient of the shortcut path, nB) so that the apply pass
     // reads ONE gradient tensor instead of gA, gB and the mask again
     RUNP(kBnBwdReduce, bn_bwd_reduce(gA, gB, B.c3.y, B.has_ds ? B.ds.y : nullptr, nullptr, nullptr, B.mask, B.c3.rows,
-                                     b3.c, net->bn_partial, &nblk, st, gB_h, gB_w, B.has_ds ? nullptr : nB));
+                                     b3.c, net->bn_partial, &nblk, st, gB_h, gB_w, B.has_ds ? nullptr : nB,
+                                     bi == hi - 1 ? g3 : nullptr));
     if (B.has_ds) {
       BNLayer& bd = B.ds.bn;
       RUNP(kBnBwdApply, bn_bwd_coeffs(net->bn_partial, nblk, kparts, 2, B.c3.rows, b3.c, bd.mean, bd.invstd,
@@ -644,6 +720,37 @@ static int backward_blocks(dirb200_net* net, int lo, int hi, const float* params
   return DIRB200_OK;
 }
 
+// The work of one backward stage (the incoming gradients are in place), graph-replayed in slot g.  The captured
+// sequence leaves host-side state behind (which scratch buffers hold the gradients entering the next stage): recorded
+// at capture, restored at replay -- the sequence of buffers is the same in every step that uses the slot.
+static int backward_stage_run(dirb200_net* net, int stage, const float* params, float* grads, const __nv_bfloat16* g3,
+                              dirb200_net::GraphSlot& g, cudaStream_t st) {
+  auto body = [&](cudaStream_t st) -> int {
+    if (stage >= 1) {
+      RUN(backward_blocks(net, net->stage_begin[stage], net->stage_begin[stage + 1], params, grads, st, g3));
+    } else {
+      // ---- stem: maxpool -> bn1+relu -> conv1 (no data gradient needed)
+      __nv_bfloat16 *t1 = net->scratch[4], *t3 = net->scratch[6];
+      RUNP(kPool, maxpool_bwd(net->bw_gA, net->bw_gB, net->pool_idx, net->n, net->stem.s.ho, net->stem.s.wo, 64, t3, st));
+      RUN(conv_bn_backward(net, net->stem, t3, params, grads, t1, st));
+      RUN(wgrad_step(net, net->x_s2d, t1, net->stem, st));
+    }
+    RUN(wgrad_reduce_stage(net, stage, grads, st));
+    return DIRB200_OK;
+  };
+  if (!graphs_enabled() || net->profiling) return body(st);
+  const bool replay = g.exec && g.k0 == params && g.k1 == grads;
+  RUN(run_graphed(net, g, params, grads, st, body));
+  if (replay) {
+    net->bw_gA = g.gA; net->bw_gB = g.gB; net->bw_nA = g.nA; net->bw_nB = g.nB; net->bw_spareB = g.spareB;
+    net->bw_gB_h = g.gB_h; net->bw_gB_w = g.gB_w;
+  } else {
+    g.gA = net->bw_gA; g.gB = net->bw_gB; g.nA = net->bw_nA; g.nB = net->bw_nB; g.spareB = net->bw_spareB;
+    g.gB_h = net->bw_gB_h; g.gB_w = net->bw_gB_w;
+  }
+  return DIRB200_OK;
+}
+
 }  // namespace dirb200
 
 extern "C" {
@@ -668,40 +775,60 @@ int dirb200_resnet_backward_stage(dirb200_net* net, int stage, const float* d_en
     net->bw_gB_h = net->bw_gB_w = 0;
     RUNP(kPool, avgpool_bwd(d_enc, net->n, net->feat_hw, net->feat_c, net->bw_gA, st));
   } else {
-    DIRB_CHECK_ARG(net->bwd_next_stage == stage, "resnet_backward_stage: stage %d out of order (expected %d)", stage,
-                   net->bwd_next_stage);
+    DIRB_CHECK_ARG(net->bwd_next_stage == stage && !net->bwd_blocks,
+                   "resnet_backward_stage: stage %d out of order (expected %d%s)", stage, net->bwd_next_stage,
+                   net->bwd_blocks ? " of a multi-scale backward" : "");
   }
   net->bwd_next_stage = -1;
-  auto body = [&](cudaStream_t st) -> int {
-    if (stage >= 1) {
-      RUN(backward_blocks(net, net->stage_begin[stage], net->stage_begin[stage + 1], params, grads, st));
-    } else {
-      // ---- stem: maxpool -> bn1+relu -> conv1 (no data gradient needed)
-      __nv_bfloat16 *t1 = net->scratch[4], *t3 = net->scratch[6];
-      RUNP(kPool, maxpool_bwd(net->bw_gA, net->bw_gB, net->pool_idx, net->n, net->stem.s.ho, net->stem.s.wo, 64, t3, st));
-      RUN(conv_bn_backward(net, net->stem, t3, params, grads, t1, st));
-      RUN(wgrad_step(net, net->x_s2d, t1, net->stem, st));
-    }
-    RUN(wgrad_reduce_stage(net, stage, grads, st));
-    return DIRB200_OK;
-  };
-  if (graphs_enabled() && !net->profiling && stage < 6) {
-    // the captured sequence leaves host-side state behind (which scratch buffers hold the gradients entering the next
-    // stage): recorded at capture, restored at replay -- the sequence of buffers is the same in every step
-    dirb200_net::GraphSlot& g = net->g_bwd[stage];
-    const bool replay = g.exec && g.k0 == params && g.k1 == grads;
-    RUN(run_graphed(net, g, params, grads, st, body));
-    if (replay) {
-      net->bw_gA = g.gA; net->bw_gB = g.gB; net->bw_nA = g.nA; net->bw_nB = g.nB; net->bw_spareB = g.spareB;
-      net->bw_gB_h = g.gB_h; net->bw_gB_w = g.gB_w;
-    } else {
-      g.gA = net->bw_gA; g.gB = net->bw_gB; g.nA = net->bw_nA; g.nB = net->bw_nB; g.spareB = net->bw_spareB;
-      g.gB_h = net->bw_gB_h; g.gB_w = net->bw_gB_w;
-    }
-  } else {
-    RUN(body(st));
-  }
+  net->bwd_blocks = false;
+  RUN(backward_stage_run(net, stage, params, grads, nullptr, net->g_bwd[stage], st));
   net->bwd_next_stage = stage - 1;          // -1 after the stem: nothing pending
+  return DIRB200_OK;
+}
+
+/* Multi-scale backward (nyud2-dir/models/modules.py:33-58, E_resnet.forward): stage = num_stages first, then
+ * num_stages-1 ... 1, then 0, after a training-mode forward.  Stage s >= 1 reads d_block, the bf16 NHWC gradient of
+ * the output of layer group s (NULL: zero); stage 0 reads nothing.  A stage that receives no gradient, neither its own
+ * nor from the stages above, does nothing: its parameter gradients keep their values. */
+int dirb200_resnet_backward_blocks_stage(dirb200_net* net, int stage, const void* d_block, const float* params,
+                                         float* grads, void* stream) {
+  DIRB_CHECK_ARG(net && params && grads, "resnet_backward_blocks_stage: null pointer");
+  const int nst = (int)net->stage_begin.size() - 2;
+  DIRB_CHECK_ARG(stage >= 0 && stage <= nst, "resnet_backward_blocks_stage: bad stage %d", stage);
+  DIRB_CHECK_ARG(stage > 0 || !d_block, "resnet_backward_blocks_stage: stage 0 (the stem) takes no block gradient");
+  RUN(check_blocks_mode(net, "resnet_backward_blocks_stage"));
+  cudaStream_t st = as_stream(stream);
+  if (stage == nst) {
+    DIRB_CHECK_ARG(net->forward_was_training, "resnet_backward_blocks_stage: needs a preceding training-mode forward");
+    net->bwd_top = -1;
+  } else {
+    DIRB_CHECK_ARG(net->bwd_next_stage == stage && net->bwd_blocks,
+                   "resnet_backward_blocks_stage: stage %d out of order (expected %d%s)", stage, net->bwd_next_stage,
+                   net->bwd_blocks ? "" : " of a multi-scale backward");
+  }
+  net->bwd_next_stage = -1;
+  net->bwd_blocks = true;
+  const __nv_bfloat16* g3 = nullptr;
+  if (stage > 0 && d_block) {
+    const Block& B = net->blocks[net->stage_begin[stage + 1] - 1];
+    const size_t bytes = sizeof(__nv_bfloat16) * (size_t)B.c3.rows * B.c3.s.cout;
+    if (net->bwd_top < 0) {
+      // the first gradient of this backward: it enters like the average-pool backward's output does
+      net->bwd_top = stage;
+      net->bw_gA = net->scratch[0]; net->bw_gB = nullptr; net->bw_nA = net->scratch[2]; net->bw_nB = net->scratch[3];
+      net->bw_spareB = net->scratch[1];
+      net->bw_gB_h = net->bw_gB_w = 0;
+      DIRB_CUDA(cudaMemcpyAsync(net->bw_gA, d_block, bytes, cudaMemcpyDeviceToDevice, st));
+    } else {
+      // a third operand of the group output's BN-backward reduction, staged at a fixed address for the graph
+      DIRB_CUDA(cudaMemcpyAsync(net->scratch[7], d_block, bytes, cudaMemcpyDeviceToDevice, st));
+      g3 = net->scratch[7];
+    }
+  }
+  if (net->bwd_top >= 0)
+    RUN(backward_stage_run(net, stage, params, grads, g3, net->g_bwd_blocks[stage][net->bwd_top][g3 ? 1 : 0], st));
+  net->bwd_next_stage = stage - 1;
+  if (stage == 0) net->bwd_blocks = false;
   return DIRB200_OK;
 }
 

@@ -6,6 +6,10 @@ linear, FDS), hence the reference's state_dict keys and shapes, the same
 `forward(x, targets=None, epoch=None)` contract (resnet.py:127-153) and the
 same initialisation (resnet.py:103-109).
 
+`E_resnet(resnet50())` is NYUD2-DIR's multi-scale encoder
+(nyud2-dir/models/modules.py:33-58): the same backbone without avgpool / fc,
+returning the four layer-group outputs as NHWC bf16 tensors.
+
 The arithmetic does not go through torch.nn: the conv/BN/ReLU/pool stack runs
 in libdirb200's native runner (wgmma implicit-GEMM convolutions + fused
 HBM-bound layers, NHWC bf16 with fp32 accumulation), the 2048->1 regressor
@@ -43,6 +47,8 @@ _lib.register({
     "dirb200_resnet_set_profiling": (c_int, [P, c_int]),
     "dirb200_resnet_read_profile": (c_int, [P, P, P]),
     "dirb200_resnet_peek": (c_int, [P, c_int, c_int, P, P, P]),
+    "dirb200_resnet_forward_blocks": (c_int, [P, P, P, P, c_int, P, P]),
+    "dirb200_resnet_backward_blocks_stage": (c_int, [P, c_int, P, P, P, P]),
     "dirb200_linear1_fwd": (c_int, [P, P, P, c_int64, c_int, P, P]),
     "dirb200_linear1_bwd": (c_int, [P, P, P, c_int64, c_int, P, P, P, P]),
     "dirb200_adam_step": (c_int, [P, P, P, P, c_int64, c_float, c_float, c_float, c_float, c_float, c_int64,
@@ -149,10 +155,39 @@ class _BackboneFn(torch.autograd.Function):
         return None, None, None
 
 
+class _EncoderFn(torch.autograd.Function):
+    """x -> the four layer-group outputs through the native runner; the backward takes a gradient for any subset of
+    them (an unused output costs nothing) and accumulates the parameter gradients into the flat gradient buffer."""
+
+    @staticmethod
+    def forward(ctx, x, anchor, model):
+        ctx.set_materialize_grads(False)
+        ctx.model = model
+        ctx.shape = tuple(x.shape)
+        return model._run_forward_blocks(x, training=True)
+
+    @staticmethod
+    def backward(ctx, *grads):
+        ctx.model._run_backward(ctx.shape, grads, blocks=True)
+        return None, None, None
+
+
+def _feature_maps(h, w, num_stages=4):
+    """(h, w) of the stem output, the max-pool output and the output of layer groups 2..num_stages for an h x w input
+    (layer1 keeps the max-pool map)."""
+    half = lambda a: (a - 1) // 2 + 1          # 3x3 / pad 1 and 1x1 / pad 0 filters at stride 2
+    maps = [(h // 2, w // 2)]
+    maps.append((half(maps[0][0]), half(maps[0][1])))
+    for _ in range(num_stages - 1):
+        maps.append((half(maps[-1][0]), half(maps[-1][1])))
+    return maps
+
+
 class ResNet(nn.Module):
 
-    def __init__(self, block, layers, fds, bucket_num, bucket_start, start_update, start_smooth,
-                 kernel, ks, sigma, momentum, dropout=None):
+    # FDS defaults as fds.FDS's, for constructions that do not use FDS (E_resnet(resnet50()))
+    def __init__(self, block, layers, fds=False, bucket_num=100, bucket_start=7, start_update=0, start_smooth=1,
+                 kernel='gaussian', ks=5, sigma=2, momentum=0.9, dropout=None):
         self.inplanes = 64
         super(ResNet, self).__init__()
         assert block is Bottleneck, "the native runner implements the bottleneck ResNets (resnet50 and deeper)"
@@ -335,24 +370,48 @@ class ResNet(nn.Module):
             self._flat["nbt"] += 1
         return enc
 
-    def _run_backward(self, shape, g):
+    def _run_forward_blocks(self, x, training):
+        """x fp32 NCHW [n, 3, h, w] -> the outputs of layer1..4, NHWC bf16 [n, h_s, w_s, 256 << s]."""
+        _lib.require_cuda(x, self._flat["params"])
+        x = x.detach().to(torch.float32).contiguous()
+        n, _, h, w = x.shape
+        net = self._net(tuple(x.shape))
+        maps = _feature_maps(h, w, len(self._layers))[1:]
+        outs = [torch.empty(n, hs, ws, 64 * Bottleneck.expansion << s, dtype=torch.bfloat16, device=x.device)
+                for s, (hs, ws) in enumerate(maps)]
+        ptrs = (c_void_p * len(outs))(*[o.data_ptr() for o in outs])
+        _lib.call("dirb200_resnet_forward_blocks", net, _lib.ptr(x), _lib.ptr(self._flat["params"]),
+                  _lib.ptr(self._flat["running"]), int(training), ptrs, _lib.stream_ptr())
+        if training:
+            self._flat["nbt"] += 1
+        return tuple(outs)
+
+    def _run_backward(self, shape, g, blocks=False):
+        """g: the encoding's gradient, or (blocks=True) one gradient (or None) per layer-group output."""
         if shape not in self._nets:
             raise _lib.Dirb200Error(f"backward for input shape {shape}: its runner (and the activations of the forward "
                                     "pass) was evicted -- more than MAX_NETS shapes ran between forward and backward")
         self._ensure_grads()
-        g = g.detach().to(torch.float32).contiguous()
+        if blocks:
+            g = [None if t is None else t.detach().to(torch.bfloat16).contiguous() for t in g]
+        else:
+            g = g.detach().to(torch.float32).contiguous()
         net = self._net(shape)
         hook = self._grad_bucket_hook
-        if hook is None:
+        if hook is None and not blocks:
             _lib.call("dirb200_resnet_backward", net, _lib.ptr(g), _lib.ptr(self._flat["params"]),
                       _lib.ptr(self._flat["grads"]), _lib.stream_ptr())
             return
         # stage by stage (layer4 ... layer1, stem); after each layer group its slice of the flat gradient is final and
         # is handed to the hook (parallel.DataParallel: an asynchronous NCCL all-reduce that overlaps the rest)
         for stage in range(_lib.raw("dirb200_resnet_num_stages")(net), -1, -1):
-            _lib.call("dirb200_resnet_backward_stage", net, stage, _lib.ptr(g), _lib.ptr(self._flat["params"]),
-                      _lib.ptr(self._flat["grads"]), _lib.stream_ptr())
-            if stage >= 1:
+            if blocks:
+                _lib.call("dirb200_resnet_backward_blocks_stage", net, stage, _lib.ptr(g[stage - 1] if stage else None),
+                          _lib.ptr(self._flat["params"]), _lib.ptr(self._flat["grads"]), _lib.stream_ptr())
+            else:
+                _lib.call("dirb200_resnet_backward_stage", net, stage, _lib.ptr(g), _lib.ptr(self._flat["params"]),
+                          _lib.ptr(self._flat["grads"]), _lib.stream_ptr())
+            if stage >= 1 and hook is not None:
                 lo, hi = c_int64(), c_int64()
                 _lib.call("dirb200_resnet_stage_param_range", net, stage, ctypes.byref(lo), ctypes.byref(hi))
                 hook(lo.value, hi.value)
@@ -383,10 +442,11 @@ class ResNet(nn.Module):
                                             version=2)
         flat = torch.as_tensor(_Arr(), device=self._flat["params"].device).view(torch.bfloat16)
         n = shape[0]
-        side = int(round((rows.value // n) ** 0.5))
+        # the net's maps have strictly decreasing pixel counts: the count identifies the map
+        h, w = next(m for m in _feature_maps(shape[2], shape[3], len(self._layers)) if m[0] * m[1] * n == rows.value)
         if not copy:
-            return flat.view(n, side, side, ch.value).permute(0, 3, 1, 2)
-        return flat.float().view(n, side, side, ch.value).permute(0, 3, 1, 2).contiguous()
+            return flat.view(n, h, w, ch.value).permute(0, 3, 1, 2)
+        return flat.float().view(n, h, w, ch.value).permute(0, 3, 1, 2).contiguous()
 
     # ---------------------------------------------------------------- forward
     def forward(self, x, targets=None, epoch=None):
@@ -422,3 +482,39 @@ class ResNet(nn.Module):
 
 def resnet50(**kwargs):
     return ResNet(Bottleneck, [3, 4, 6, 3], **kwargs)
+
+
+class E_resnet(nn.Module):
+    """NYUD2-DIR's encoder (nyud2-dir/models/modules.py:33-58): `original_model`'s stem and layer1..4 without avgpool /
+    linear.  It shares the native ResNet's holders, flat parameter / gradient / running-statistics buffers and runner
+    cache, so its state_dict has the reference E_resnet's keys and loads a torchvision-layout ResNet-50 checkpoint.
+
+    forward(x): x fp32 NCHW [B, 3, H, W] (H, W multiples of 4) -> (x_block1, x_block2, x_block3, x_block4), NHWC bf16
+    [B, h_s, w_s, C_s] with C_s = 256, 512, 1024, 2048 (the layout dense_ops consumes).  In training mode with
+    gradients enabled they carry autograd history into the backbone parameters; x receives no gradient."""
+
+    def __init__(self, original_model, num_features=2048):
+        super(E_resnet, self).__init__()
+        assert isinstance(original_model, ResNet), "E_resnet wraps the native resnet.ResNet"
+        object.__setattr__(self, "_resnet", original_model)      # not a submodule: no linear / FDS keys
+        self.conv1 = original_model.conv1
+        self.bn1 = original_model.bn1
+        self.layer1 = original_model.layer1
+        self.layer2 = original_model.layer2
+        self.layer3 = original_model.layer3
+        self.layer4 = original_model.layer4
+
+    def _apply(self, fn, *args, **kwargs):
+        # device / dtype moves go through the owning ResNet, which rebuilds its flat buffers and views (ResNet._apply)
+        self._resnet._apply(fn, *args, **kwargs)
+        return self
+
+    def forward(self, x):
+        m = self._resnet
+        if self.training and torch.is_grad_enabled():
+            lw = m.linear.weight
+            if m._grad_views is None or lw.grad is None or lw.grad.data_ptr() != m._grad_views[-2].data_ptr():
+                m._ensure_grads()
+            if any(p.requires_grad for p in m._flat_param_list()[:-2]):
+                return _EncoderFn.apply(x, m._anchor, m)
+        return m._run_forward_blocks(x, training=self.training)

@@ -336,6 +336,9 @@ int dirb200_bn_bwd_coeffs_layout(const float* partial, const int* layout_host, i
  * BN in the same order as (running_mean, running_var). */
 typedef struct dirb200_net dirb200_net;
 
+/* H and W: multiples of 4 (the input space-to-depth needs even H, W; the max-pool backward an even stem output), at
+ * most 1024 (the convolutions pack a stem-output row / column in 9 bits); N at most 8192 (13 bits of image index),
+ * and N * H/2 * W/2 < 2^31. */
 int dirb200_resnet_create(int n, int h, int w, const int* blocks_per_stage, int num_stages, dirb200_net** out);
 void dirb200_resnet_destroy(dirb200_net* net);
 int64_t dirb200_resnet_param_count(const dirb200_net* net);   /* floats in the flat parameter buffer */
@@ -360,6 +363,21 @@ int dirb200_resnet_num_stages(const dirb200_net* net);
 int dirb200_resnet_backward_stage(dirb200_net* net, int stage, const float* d_enc, const float* params, float* grads,
                                   void* stream);
 int dirb200_resnet_stage_param_range(const dirb200_net* net, int stage, int64_t* lo, int64_t* hi);
+
+/* Multi-scale encoder forward (nyud2-dir/models/modules.py:33-58, E_resnet.forward): the forward above without the
+ * average pool; block_out[s] receives the output of the last block of layer group s+1 as NHWC bf16 [n, h_s, w_s, C_s]
+ * (256 / 512 / 1024 / 2048 channels for ResNet-50).  training == 0: running statistics (folded-BN forward).  Every layer
+ * group must end in an identity block (true of ResNet-50 and deeper). */
+int dirb200_resnet_forward_blocks(dirb200_net* net, const float* x_nchw, const float* params, float* bn_running,
+                                  int training, void* const* block_out, void* stream);
+
+/* Its backward (nyud2-dir/models/modules.py:33-58, E_resnet.forward), one stage per call in the order of
+ * dirb200_resnet_backward_stage: stage num_stages, ..., 1, then 0 (stem), after a training-mode forward.  Stage s >= 1
+ * reads d_block, the NHWC bf16 gradient of block_out[s-1], or nothing when it is NULL; stage 0 reads nothing.
+ * ACCUMULATES into grads, with the same per-stage parameter ranges.  A stage that receives no gradient, neither its own
+ * nor from a stage above, does nothing (its parameter gradients keep their values). */
+int dirb200_resnet_backward_blocks_stage(dirb200_net* net, int stage, const void* d_block, const float* params,
+                                         float* grads, void* stream);
 
 /* Per-kernel-class device timing of forward/backward (CUDA events around every launch group).  Classes:
  * 0 prep (weight re-layout, s2d), 1 conv fprop, 2 conv dgrad, 3 conv wgrad GEMM, 4 wgrad split-K reduce,

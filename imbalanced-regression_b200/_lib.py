@@ -67,6 +67,14 @@ _SIGS = {
     "dirb200_maxpool3x3s2_bwd": (c_int, [P, P, c_int, c_int, c_int, c_int, P, P]),
     "dirb200_avgpool_fwd": (c_int, [P, c_int, c_int, c_int, P, P]),
     "dirb200_avgpool_bwd": (c_int, [P, c_int, c_int, c_int, P, P]),
+    # test aids: the BatchNorm / pooling layer kernels one launch at a time
+    "dirb200_layer_bn_stats": (c_int, [P, c_int64, c_int, P, P, P]),
+    "dirb200_layer_bn_apply": (c_int, [P, P, P, P, P, P, P, c_int, c_int64, c_int, P, P, P]),
+    "dirb200_layer_bn_bwd_reduce": (c_int, [P, P, P, P, P, P, P, P, c_int64, c_int, c_int, c_int, P, P, P, P]),
+    "dirb200_layer_bn_bwd_coeffs": (c_int, [P, c_int, c_int, c_int, c_int64, c_int, P, P, P, P, P, P, P]),
+    "dirb200_layer_bn_bwd_apply": (c_int, [P, P, P, P, P, P, P, P, P, c_int64, c_int, c_int, c_int, P, P, P, P]),
+    "dirb200_layer_bn_relu_maxpool_fwd": (c_int, [P, P, P, c_int, c_int, c_int, c_int, P, P, P]),
+    "dirb200_layer_maxpool_bwd": (c_int, [P, P, P, c_int, c_int, c_int, c_int, P, P]),
     "dirb200_upsample_bilinear_fwd": (c_int, [P, c_int, c_int, c_int, c_int, c_int, c_int, P, P]),
     "dirb200_upsample_bilinear_bwd": (c_int, [P, c_int, c_int, c_int, c_int, c_int, c_int, P, P]),
     "dirb200_copy_channels": (c_int, [P, c_int, c_int, P, c_int, c_int, c_int, c_int64, P]),

@@ -984,9 +984,20 @@ static int resident_ctas(K kernel, size_t smem) {
 }
 
 // ------------------------------------------------------------- host wrappers
+// Channel counts of the row-walking BN kernels: a CTA's 256 threads are (c / 8 channel groups) x (row lanes), so c / 8
+// must divide 256: c = 8, 16, 32, ..., 2048.  Tested before anything divides by c / 8.
+static inline bool bn_channels_ok(int c) { return c >= 8 && c % 8 == 0 && 256 % (c / 8) == 0; }
+// Compact second gradient (g2_h, g2_w > 0): even maps that tile the rows; CompactG2::locate divides 32-bit row indices.
+static inline bool compact_ok(int g2_h, int g2_w, int64_t rows) {
+  if (g2_h == 0 && g2_w == 0) return true;
+  return g2_h > 0 && g2_w > 0 && g2_h % 2 == 0 && g2_w % 2 == 0 && rows < (int64_t(1) << 31) &&
+         rows % ((int64_t)g2_h * g2_w) == 0;
+}
+
 int bn_stats(const __nv_bfloat16* y, int64_t rows, int c, float* partial, int* nblocks, cudaStream_t st) {
+  DIRB_CHECK_ARG(bn_channels_ok(c), "bn_stats: unsupported channel count %d (8, 16, 32, ..., 2048)", c);
+  DIRB_CHECK_ARG(rows > 0, "bn_stats: rows must be positive");
   const int cgroups = c / 8;
-  DIRB_CHECK_ARG(c % 8 == 0 && cgroups <= 256 && 256 % cgroups == 0, "bn_stats: unsupported channel count %d", c);
   const int lanes = 256 / cgroups;
   *nblocks = reduce_grid(rows, lanes);
   bn_stats_kernel<<<*nblocks, 256, 256 * 16 * sizeof(float), st>>>(y, rows, c, partial);
@@ -1023,9 +1034,12 @@ int bn_eval_coeffs_all(const BnEvalDesc* descs_dev, int nlayers, int max_c, cons
 int bn_apply(const __nv_bfloat16* y, const float* scale, const float* shift, const __nv_bfloat16* res,
              const __nv_bfloat16* res_y, const float* res_scale, const float* res_shift, bool relu, int64_t rows, int c,
              __nv_bfloat16* out, uint8_t* mask_out, cudaStream_t st) {
+  DIRB_CHECK_ARG(bn_channels_ok(c), "bn_apply: unsupported channel count %d (8, 16, 32, ..., 2048)", c);
+  DIRB_CHECK_ARG(rows > 0, "bn_apply: rows must be positive");
   const int cgroups = c / 8;
-  DIRB_CHECK_ARG(c % 8 == 0 && cgroups <= 256 && 256 % cgroups == 0, "bn_apply: unsupported channel count %d", c);
   DIRB_CHECK_ARG(!(res && res_y), "bn_apply: one shortcut operand (identity or the downsample branch's raw output)");
+  // the mask bit tests the stored value for a non-zero magnitude: that is "> 0" only behind the ReLU
+  DIRB_CHECK_ARG(!mask_out || relu, "bn_apply: the ReLU mask needs relu");
   const int want = stream_grid(rows, 256 / cgroups);
 #define DIRB_BNA(RES, RESY, MASK)                                                                                 \
   do {                                                                                                            \
@@ -1064,10 +1078,11 @@ int bn_bwd_reduce(const __nv_bfloat16* g1, const __nv_bfloat16* g2, const __nv_b
                   int* nblocks, cudaStream_t st, int g2_h, int g2_w, __nv_bfloat16* dz_out, const __nv_bfloat16* g3) {
   const CompactG2 cg2 = make_compact(g2_h, g2_w);
   DIRB_CHECK_ARG(!g3 || (g2 && dz_out), "bn_bwd_reduce: a third gradient is added in the two-gradient identity forms only");
-  DIRB_CHECK_ARG(g2_h == 0 || (g2 && mask && !y2 && g2_h % 2 == 0 && g2_w % 2 == 0 && rows % ((int64_t)g2_h * g2_w) == 0),
+  DIRB_CHECK_ARG(bn_channels_ok(c), "bn_bwd_reduce: unsupported channel count %d (8, 16, 32, ..., 2048)", c);
+  DIRB_CHECK_ARG(rows > 0, "bn_bwd_reduce: rows must be positive");
+  DIRB_CHECK_ARG(compact_ok(g2_h, g2_w, rows) && (g2_h == 0 || (g2 && mask && !y2)),
                  "bn_bwd_reduce: bad compact second gradient");
   const int cgroups = c / 8;
-  DIRB_CHECK_ARG(c % 8 == 0 && cgroups <= 256 && 256 % cgroups == 0, "bn_bwd_reduce: unsupported channel count %d", c);
   DIRB_CHECK_ARG(mask || (!g2 && !y2 && (scale != nullptr) == (shift != nullptr)),
                  "bn_bwd_reduce: the mask-from-y and the no-ReLU forms take one gradient, one BN");
   DIRB_CHECK_ARG(!dz_out || (mask && !y2), "bn_bwd_reduce: dz is stored for identity blocks only");
@@ -1125,9 +1140,11 @@ int bn_bwd_apply(const __nv_bfloat16* g1, const __nv_bfloat16* g2, const __nv_bf
                  const uint8_t* mask, int64_t rows, int c, __nv_bfloat16* dy, __nv_bfloat16* dy2,
                  __nv_bfloat16* dz_out, cudaStream_t st, int g2_h, int g2_w) {
   const CompactG2 cg2 = make_compact(g2_h, g2_w);
-  DIRB_CHECK_ARG(g2_h == 0 || (g2 && mask && !y2 && dz_out), "bn_bwd_apply: bad compact second gradient");
+  DIRB_CHECK_ARG(bn_channels_ok(c), "bn_bwd_apply: unsupported channel count %d (8, 16, 32, ..., 2048)", c);
+  DIRB_CHECK_ARG(rows > 0, "bn_bwd_apply: rows must be positive");
+  DIRB_CHECK_ARG(compact_ok(g2_h, g2_w, rows) && (g2_h == 0 || (g2 && mask && !y2 && dz_out)),
+                 "bn_bwd_apply: bad compact second gradient");
   const int cgroups = c / 8;
-  DIRB_CHECK_ARG(c % 8 == 0 && cgroups <= 256 && 256 % cgroups == 0, "bn_bwd_apply: unsupported channel count %d", c);
   DIRB_CHECK_ARG(mask || (!g2 && !y2 && !dz_out && (scale != nullptr) == (shift != nullptr)),
                  "bn_bwd_apply: the mask-from-y and the dz-input forms take one gradient, one BN");
   DIRB_CHECK_ARG(!(y2 && dz_out), "bn_bwd_apply: a block has either a downsample branch or an identity path");
@@ -1202,8 +1219,10 @@ size_t dirb200_bn_workspace_bytes(int c) { return sizeof(float) * static_cast<si
 int dirb200_bn_train_fwd(const void* y, int64_t rows, int c, const float* gamma, const float* beta, float eps,
                          float momentum, float* running_mean, float* running_var, int relu, void* out, float* save_mean,
                          float* save_invstd, float* scale_shift, void* workspace, void* stream) {
-  DIRB_CHECK_ARG(y && out && gamma && beta && save_mean && save_invstd && scale_shift && workspace && rows > 0,
+  DIRB_CHECK_ARG(y && out && gamma && beta && save_mean && save_invstd && scale_shift && workspace,
                  "bn_train_fwd: null pointer");
+  DIRB_CHECK_ARG(bn_channels_ok(c), "bn_train_fwd: unsupported channel count %d (8, 16, 32, ..., 2048)", c);
+  DIRB_CHECK_ARG(rows > 0, "bn_train_fwd: rows must be positive");
   cudaStream_t st = as_stream(stream);
   float* partial = static_cast<float*>(workspace);
   int nblk = 0;
@@ -1219,8 +1238,11 @@ int dirb200_bn_train_bwd(const void* grad_out, const void* y, int64_t rows, int 
                          const float* save_mean, const float* save_invstd, const float* scale_shift, int relu,
                          float* grad_gamma, float* grad_beta, void* grad_y, void* workspace, void* stream) {
   DIRB_CHECK_ARG(grad_out && y && gamma && save_mean && save_invstd && grad_gamma && grad_beta && grad_y && workspace &&
-                     rows > 0 && (!relu || scale_shift),
+                     (!relu || scale_shift),
                  "bn_train_bwd: null pointer");
+  // before bn_partial_floats(c) below: it queries the device
+  DIRB_CHECK_ARG(bn_channels_ok(c), "bn_train_bwd: unsupported channel count %d (8, 16, 32, ..., 2048)", c);
+  DIRB_CHECK_ARG(rows > 0, "bn_train_bwd: rows must be positive");
   cudaStream_t st = as_stream(stream);
   float* partial = static_cast<float*>(workspace);
   float* coef = partial + bn_partial_floats(c) - 3 * c;        // the reduction uses at most 2/3 of the buffer
@@ -1257,6 +1279,75 @@ int dirb200_bn_bwd_coeffs_layout(const float* partial, const int* layout_host, i
   const StatLayout lay{layout_host[0], layout_host[1], layout_host[2], layout_host[3]};
   return bn_bwd_coeffs_layout(partial, lay, rows, c, mean, invstd, gamma, grad_gamma, grad_beta, coef_out,
                               as_stream(stream));
+}
+
+/* ---- Test aids: the BatchNorm / pooling layer kernels, one launch each (see include/dirb200.h).  The internal
+ * wrappers refuse unsupported channel counts, row counts and operand combinations before their first CUDA call; these
+ * add the pointer checks. */
+using bf16 = __nv_bfloat16;
+
+int dirb200_layer_bn_stats(const void* y, int64_t rows, int c, float* partial, int* nblocks_host, void* stream) {
+  DIRB_CHECK_ARG(y && partial && nblocks_host, "layer_bn_stats: null pointer");
+  return bn_stats(static_cast<const bf16*>(y), rows, c, partial, nblocks_host, as_stream(stream));
+}
+
+int dirb200_layer_bn_apply(const void* y, const float* scale, const float* shift, const void* res, const void* res_y,
+                           const float* res_scale, const float* res_shift, int relu, int64_t rows, int c, void* out,
+                           uint8_t* mask_out, void* stream) {
+  DIRB_CHECK_ARG(y && scale && shift && out, "layer_bn_apply: null pointer");
+  DIRB_CHECK_ARG(!res_y || (res_scale && res_shift), "layer_bn_apply: res_y needs res_scale and res_shift");
+  return bn_apply(static_cast<const bf16*>(y), scale, shift, static_cast<const bf16*>(res), static_cast<const bf16*>(res_y),
+                  res_scale, res_shift, relu != 0, rows, c, static_cast<bf16*>(out), mask_out, as_stream(stream));
+}
+
+int dirb200_layer_bn_bwd_reduce(const void* g1, const void* g2, const void* g3, const void* y, const void* y2,
+                                const float* scale, const float* shift, const uint8_t* mask, int64_t rows, int c,
+                                int g2_h, int g2_w, void* dz_out, float* partial, int* nblocks_host, void* stream) {
+  DIRB_CHECK_ARG(g1 && y && partial && nblocks_host, "layer_bn_bwd_reduce: null pointer");
+  return bn_bwd_reduce(static_cast<const bf16*>(g1), static_cast<const bf16*>(g2), static_cast<const bf16*>(y),
+                       static_cast<const bf16*>(y2), scale, shift, mask, rows, c, partial, nblocks_host,
+                       as_stream(stream), g2_h, g2_w, static_cast<bf16*>(dz_out), static_cast<const bf16*>(g3));
+}
+
+int dirb200_layer_bn_bwd_coeffs(const float* partial, int nblocks, int k, int gslot, int64_t rows, int c,
+                                const float* mean, const float* invstd, const float* gamma, float* grad_gamma,
+                                float* grad_beta, float* coef_out, void* stream) {
+  DIRB_CHECK_ARG(partial && mean && invstd && gamma && grad_gamma && grad_beta && coef_out,
+                 "layer_bn_bwd_coeffs: null pointer");
+  DIRB_CHECK_ARG(bn_channels_ok(c), "layer_bn_bwd_coeffs: unsupported channel count %d (8, 16, 32, ..., 2048)", c);
+  DIRB_CHECK_ARG(rows > 0 && nblocks > 0, "layer_bn_bwd_coeffs: rows and nblocks must be positive");
+  DIRB_CHECK_ARG((k == 2 || k == 3) && gslot >= 1 && gslot < k, "layer_bn_bwd_coeffs: K must be 2 or 3, 1 <= gslot < K");
+  return bn_bwd_coeffs(partial, nblocks, k, gslot, rows, c, mean, invstd, gamma, grad_gamma, grad_beta, coef_out,
+                       as_stream(stream));
+}
+
+int dirb200_layer_bn_bwd_apply(const void* g1, const void* g2, const void* y, const float* coef, const void* y2,
+                               const float* coef2, const float* scale, const float* shift, const uint8_t* mask,
+                               int64_t rows, int c, int g2_h, int g2_w, void* dy, void* dy2, void* dz_out,
+                               void* stream) {
+  DIRB_CHECK_ARG(g1 && y && coef && dy, "layer_bn_bwd_apply: null pointer");
+  DIRB_CHECK_ARG(!y2 || (coef2 && dy2), "layer_bn_bwd_apply: y2 needs coef2 and dy2");
+  return bn_bwd_apply(static_cast<const bf16*>(g1), static_cast<const bf16*>(g2), static_cast<const bf16*>(y), coef,
+                      static_cast<const bf16*>(y2), coef2, scale, shift, mask, rows, c, static_cast<bf16*>(dy),
+                      static_cast<bf16*>(dy2), static_cast<bf16*>(dz_out), as_stream(stream), g2_h, g2_w);
+}
+
+int dirb200_layer_bn_relu_maxpool_fwd(const void* y, const float* scale, const float* shift, int n, int h, int w, int c,
+                                      void* out, uint8_t* argmax, void* stream) {
+  DIRB_CHECK_ARG(y && scale && shift && out && argmax, "layer_bn_relu_maxpool_fwd: null pointer");
+  DIRB_CHECK_ARG(n > 0 && h > 0 && w > 0, "layer_bn_relu_maxpool_fwd: bad map size");
+  DIRB_CHECK_ARG(c > 0 && c % 8 == 0, "layer_bn_relu_maxpool_fwd: unsupported channel count %d (a multiple of 8)", c);
+  return bn_relu_maxpool_fwd(static_cast<const bf16*>(y), scale, shift, n, h, w, c, static_cast<bf16*>(out), argmax,
+                             as_stream(stream));
+}
+
+int dirb200_layer_maxpool_bwd(const void* g1, const void* g2, const uint8_t* argmax, int n, int h, int w, int c,
+                              void* dx, void* stream) {
+  DIRB_CHECK_ARG(g1 && argmax && dx, "layer_maxpool_bwd: null pointer");
+  DIRB_CHECK_ARG(n > 0 && h > 0 && w > 0, "layer_maxpool_bwd: bad map size");
+  DIRB_CHECK_ARG(c > 0 && c % 8 == 0, "layer_maxpool_bwd: unsupported channel count %d (a multiple of 8)", c);
+  return maxpool_bwd(static_cast<const bf16*>(g1), static_cast<const bf16*>(g2), argmax, n, h, w, c,
+                     static_cast<bf16*>(dx), as_stream(stream));
 }
 
 int dirb200_maxpool3x3s2_fwd(const void* x, int n, int h, int w, int c, void* out, uint8_t* argmax, void* stream) {

@@ -164,8 +164,9 @@ class _BNTrainFn(torch.autograd.Function):
 
 
 def batch_norm_train(x, weight, bias, running_mean=None, running_var=None, momentum=0.1, eps=1e-5, relu=False):
-    """nn.BatchNorm2d(training) [+ ReLU] on an NHWC bf16 tensor (channels a multiple of 8, <= 2048); running statistics
-    updated in place like torch's."""
+    """nn.BatchNorm2d(training) [+ ReLU] on an NHWC bf16 tensor (channels 8, 16, 32, ..., 2048: the BN kernels split a
+    CTA's 256 threads into channel groups of 8, so e.g. 24 channels are refused); running statistics updated in place
+    like torch's."""
     return _BNTrainFn.apply(x, weight, bias, running_mean, running_var, momentum, eps, relu)
 
 

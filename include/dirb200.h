@@ -168,7 +168,8 @@ int dirb200_lds_table_lookup(const float* values, int64_t n, float mult, int max
                              float* weights_out, void* stream);
 
 /* ------------------------------------------------ BatchNorm / pooling layers ---- */
-/* nn.BatchNorm2d in training mode on an NHWC bf16 tensor y [rows][c] (rows = N*H*W; c a multiple of 8, <= 2048),
+/* nn.BatchNorm2d in training mode on an NHWC bf16 tensor y [rows][c] (rows = N*H*W > 0; c = 8, 16, 32, ..., 2048:
+ * c / 8 channel groups must divide a CTA's 256 threads, so e.g. c = 24 is refused),
  * optionally followed by ReLU (agedb-dir/resnet.py:46-51,128-130; nyud2-dir/models/modules.py:13-21): batch statistics
  * (biased variance) -> running statistics updated in place with `momentum` (unbiased variance; NULL: not tracked) ->
  * out = [relu](gamma * (y - mean) * invstd + beta).  save_mean / save_invstd [c] and scale_shift [2][c] are kept for
@@ -323,6 +324,50 @@ int dirb200_bn_finalize_layout(const float* partial, const int* layout_host, int
 int dirb200_bn_bwd_coeffs_layout(const float* partial, const int* layout_host, int64_t rows, int c, const float* mean,
                                  const float* invstd, const float* gamma, float* grad_gamma, float* grad_beta,
                                  float* coef_out, void* stream);
+
+/* ------------------------------------------------ Test aids: BatchNorm / pooling layer kernels ---- */
+/* The HBM-bound layer kernels the runner and the BatchNorm entry points above sequence, one launch per call with the
+ * runner's own dispatch, so that each can be checked against a high-precision reference.  y, g*, res*, dz, dy*: NHWC
+ * bf16 [rows][c]; c = 8, 16, 32, ..., 2048 (c / 8 must divide 256), rows > 0.  A CTA walks rows with lanes = 256 / (c/8)
+ * row lanes per channel group; the column reductions write ONE fp32 row per CTA, partial [nblocks][K][c], at most
+ * 4 x SMs rows (nblocks returned through nblocks_host).  Masks: [rows][c/8] bytes, bit j of byte (r, g) = element
+ * (r, 8g + j) was > 0 after the ReLU. */
+
+/* Slot 0 = sum y, slot 1 = sum y^2 (K = 2); dirb200_bn_finalize_layout with layout {nblocks, 1, c, 1} consumes them. */
+int dirb200_layer_bn_stats(const void* y, int64_t rows, int c, float* partial, int* nblocks_host, void* stream);
+/* out = [relu](fma(y, scale, shift) [+ res] [+ fma(res_y, res_scale, res_shift)]) in fp32, rounded once to bf16; at most
+ * one of res / res_y.  mask_out (NULL: none; relu only) = the bits of the stored out. */
+int dirb200_layer_bn_apply(const void* y, const float* scale, const float* shift, const void* res, const void* res_y,
+                           const float* res_scale, const float* res_shift, int relu, int64_t rows, int c, void* out,
+                           uint8_t* mask_out, void* stream);
+/* BN backward moments.  dz = m * (g1 [+ g2] [+ g3]) summed in fp32 in that order; m = [fma(y, scale, shift) > 0] when
+ * mask is NULL and scale / shift are given, the stored bit when mask is given, 1 when all three are NULL.  g2 / y2 /
+ * dz_out / g3 need the mask; g3 needs g2 and dz_out; g2_h, g2_w > 0 (even, g2_h * g2_w dividing rows): g2 is the compact
+ * [rows / (g2_h g2_w)][g2_h / 2][g2_w / 2][c] gradient added at even (y, x) of the g2_h x g2_w maps, not with y2.
+ * dz_out (not with y2): dz rounded to bf16 and stored, the sums then taken over the stored values.  Slots: 0 = sum dz,
+ * 1 = sum dz*y, 2 = sum dz*y2 (K = 3 with y2, else 2). */
+int dirb200_layer_bn_bwd_reduce(const void* g1, const void* g2, const void* g3, const void* y, const void* y2,
+                                const float* scale, const float* shift, const uint8_t* mask, int64_t rows, int c,
+                                int g2_h, int g2_w, void* dz_out, float* partial, int* nblocks_host, void* stream);
+/* From those rows (K = 2 or 3): dbeta = sum of slot 0, dgamma = invstd * (sum of slot gslot - mean * dbeta), both
+ * ACCUMULATED into grad_gamma / grad_beta; coef_out [3][c] = A, B, C of dy = A*dz + B*y + C. */
+int dirb200_layer_bn_bwd_coeffs(const float* partial, int nblocks, int k, int gslot, int64_t rows, int c,
+                                const float* mean, const float* invstd, const float* gamma, float* grad_gamma,
+                                float* grad_beta, float* coef_out, void* stream);
+/* dy = bf16(fma(A, dz, fma(B, y, C))) with dz formed as in dirb200_layer_bn_bwd_reduce (no g3) and the coefficients
+ * coef [3][c]; with y2, dy2 the same from (coef2, y2); dz_out (mask forms only, not with y2): dz stored.  g1 is dz
+ * itself when mask, scale and shift are all NULL.  Compact g2 only together with dz_out. */
+int dirb200_layer_bn_bwd_apply(const void* g1, const void* g2, const void* y, const float* coef, const void* y2,
+                               const float* coef2, const float* scale, const float* shift, const uint8_t* mask,
+                               int64_t rows, int c, int g2_h, int g2_w, void* dy, void* dy2, void* dz_out,
+                               void* stream);
+/* The stem's fused relu(bn(y)) + 3x3 / stride 2 / pad 1 max pool (c a multiple of 8): out = the pool of
+ * bf16(relu(fma(y, scale, shift))), argmax = r*3+s of the first maximum in the window. */
+int dirb200_layer_bn_relu_maxpool_fwd(const void* y, const float* scale, const float* shift, int n, int h, int w, int c,
+                                      void* out, uint8_t* argmax, void* stream);
+/* dirb200_maxpool3x3s2_bwd with a second gradient g2 of the pool output (NULL: none) added in fp32 to g1. */
+int dirb200_layer_maxpool_bwd(const void* g1, const void* g2, const uint8_t* argmax, int n, int h, int w, int c,
+                              void* dx, void* stream);
 
 /* ------------------------------------------------ ResNet backbone runner ---- */
 /* Opaque native runner of the bottleneck ResNet of agedb-dir/resnet.py:41-70,

@@ -3,6 +3,7 @@
 //   torch.cat(..., 1)                      (modules.py:120: channel concat of the four MFF branches)  = a strided copy
 // The convolutions themselves (5x5 / 3x3 / 1x1) are the wgmma implicit-GEMM kernels of conv_igemm.cu.
 #include "common.cuh"
+#include "upsample.cuh"
 
 namespace dirb200 {
 
@@ -33,17 +34,6 @@ __device__ __forceinline__ void st8(__nv_bfloat16* p, const V8f& a) {
   *reinterpret_cast<uint4*>(p) = u;
 }
 
-// source index of ATen's upsample_bilinear2d with align_corners = false: max(scale * (dst + 0.5) - 0.5, 0), scale =
-// in / out (float); i0 = floor, i1 = min(i0 + 1, in - 1), lambda1 = src - i0
-__device__ __forceinline__ void src_index(int dst, float scale, int in_size, int& i0, int& i1, float& l1) {
-  float s = scale * (static_cast<float>(dst) + 0.5f) - 0.5f;
-  if (s < 0.f) s = 0.f;
-  i0 = static_cast<int>(s);
-  if (i0 > in_size - 1) i0 = in_size - 1;
-  i1 = i0 + (i0 < in_size - 1 ? 1 : 0);
-  l1 = s - static_cast<float>(i0);
-}
-
 __global__ void __launch_bounds__(256)
 upsample_bilinear_fwd_kernel(const __nv_bfloat16* __restrict__ x, int n, int h, int w, int c, int ho, int wo,
                              float sh, float sw, __nv_bfloat16* __restrict__ out) {
@@ -58,16 +48,15 @@ upsample_bilinear_fwd_kernel(const __nv_bfloat16* __restrict__ x, int n, int h, 
     const int b = static_cast<int>(t / ho);
     int y0, y1, x0, x1;
     float ly, lx;
-    src_index(oy, sh, h, y0, y1, ly);
-    src_index(ox, sw, w, x0, x1, lx);
+    upsample_src_index(oy, sh, h, y0, y1, ly);
+    upsample_src_index(ox, sw, w, x0, x1, lx);
     const __nv_bfloat16* base = x + static_cast<int64_t>(b) * h * w * c + g * 8;
     const V8f v00 = ld8(base + (static_cast<int64_t>(y0) * w + x0) * c), v01 = ld8(base + (static_cast<int64_t>(y0) * w + x1) * c);
     const V8f v10 = ld8(base + (static_cast<int64_t>(y1) * w + x0) * c), v11 = ld8(base + (static_cast<int64_t>(y1) * w + x1) * c);
-    const float hy = 1.f - ly, hx = 1.f - lx;
+    const float hy = __fsub_rn(1.f, ly), hx = __fsub_rn(1.f, lx);
     V8f o;
 #pragma unroll
-    for (int j = 0; j < 8; ++j)       // ATen's association: h0 * (w0 * v00 + w1 * v01) + h1 * (w0 * v10 + w1 * v11)
-      o.v[j] = hy * (hx * v00.v[j] + lx * v01.v[j]) + ly * (hx * v10.v[j] + lx * v11.v[j]);
+    for (int j = 0; j < 8; ++j) o.v[j] = upsample_lerp(v00.v[j], v01.v[j], v10.v[j], v11.v[j], hx, lx, hy, ly);
     st8(out + ((static_cast<int64_t>(b) * ho + oy) * wo + ox) * c + g * 8, o);
   }
 }
@@ -75,7 +64,7 @@ upsample_bilinear_fwd_kernel(const __nv_bfloat16* __restrict__ x, int n, int h, 
 // Backward as a GATHER (deterministic; ATen scatters with atomics): input pixel (iy, ix) collects w_y * w_x * dy from every
 // output pixel whose two source rows / columns include it.  Candidate output rows are those with source position in
 // (iy - 1, iy + 1): oy in [ (iy - 1 + 0.5) / sh - 0.5, (iy + 1 + 0.5) / sh - 0.5 ], widened by one and re-checked
-// exactly with src_index.
+// exactly with upsample_src_index.
 __device__ __forceinline__ void candidates(int i, float scale, int out_size, int& lo, int& hi) {
   const float inv = 1.f / scale;
   lo = static_cast<int>(floorf((static_cast<float>(i) - 0.5f) * inv - 0.5f)) - 1;
@@ -104,13 +93,13 @@ upsample_bilinear_bwd_kernel(const __nv_bfloat16* __restrict__ dy, int n, int h,
     for (int oy = ylo; oy <= yhi; ++oy) {
       int y0, y1;
       float ly;
-      src_index(oy, sh, h, y0, y1, ly);
+      upsample_src_index(oy, sh, h, y0, y1, ly);
       const float wy = (y0 == iy ? 1.f - ly : 0.f) + (y1 == iy ? ly : 0.f);
       if (wy == 0.f) continue;
       for (int ox = xlo; ox <= xhi; ++ox) {
         int x0, x1;
         float lx;
-        src_index(ox, sw, w, x0, x1, lx);
+        upsample_src_index(ox, sw, w, x0, x1, lx);
         const float wx = (x0 == ix ? 1.f - lx : 0.f) + (x1 == ix ? lx : 0.f);
         if (wx == 0.f) continue;
         const V8f gq = ld8(base + (static_cast<int64_t>(oy) * wo + ox) * c);

@@ -1258,6 +1258,13 @@ int dirb200_bn_train_bwd(const void* grad_out, const void* y, int64_t rows, int 
                       nullptr, nullptr, sc, sh, nullptr, rows, c, static_cast<__nv_bfloat16*>(grad_y), nullptr, nullptr, st);
 }
 
+int dirb200_bn_eval_coeffs(int c, const float* gamma, const float* beta, float eps, const float* running_mean,
+                           const float* running_var, float* scale, float* shift, void* stream) {
+  DIRB_CHECK_ARG(gamma && beta && running_mean && running_var && scale && shift, "bn_eval_coeffs: null pointer");
+  DIRB_CHECK_ARG(c > 0, "bn_eval_coeffs: c must be positive");
+  return bn_eval_coeffs(c, gamma, beta, eps, running_mean, running_var, scale, shift, as_stream(stream));
+}
+
 /* ---- Test aids: the consumers of the per-CTA rows the conv epilogues write (see include/dirb200.h). */
 int dirb200_bn_finalize_layout(const float* partial, const int* layout_host, int64_t rows, int c, const float* gamma,
                                const float* beta, float eps, float momentum, float* running_mean, float* running_var,

@@ -78,6 +78,10 @@ _SIGS = {
     "dirb200_upsample_bilinear_fwd": (c_int, [P, c_int, c_int, c_int, c_int, c_int, c_int, P, P]),
     "dirb200_upsample_bilinear_bwd": (c_int, [P, c_int, c_int, c_int, c_int, c_int, c_int, P, P]),
     "dirb200_copy_channels": (c_int, [P, c_int, c_int, P, c_int, c_int, c_int, c_int64, P]),
+    "dirb200_depth_head_fwd": (c_int, [P, P, P, P, c_int, c_int, c_int, c_int, P]),
+    "dirb200_depth_head_dgrad": (c_int, [P, P, P, c_int, c_int, c_int, c_int, P]),
+    "dirb200_depth_head_wgrad_workspace_bytes": (c_size_t, [c_int, c_int, c_int, c_int]),
+    "dirb200_depth_head_wgrad": (c_int, [P, P, P, P, P, c_size_t, c_int, c_int, c_int, c_int, P]),
     "dirb200_augment_batch": (c_int, [P, P, P, c_int, c_int, c_int, c_float, c_float, P, P]),
 }
 

@@ -8,6 +8,8 @@
   batch_norm_train(x, weight, bias, ...)    nn.BatchNorm2d in training mode [+ ReLU] (modules.py:13-21, 65, 109, 137-141)
   conv5x5_upsampled(x, weight, size)        conv(F.upsample(x, size), weight), 5x5 / stride 1 / pad 2 (modules.py:24-27):
                                             the up-sampled operand is formed inside the conv and never stored
+  depth_head(x, weight, bias)               R's 1-channel 5x5 conv2 with bias (modules.py:145, 169): its own memory-bound
+                                            kernels, fp32 output
 
 and the modules UpProjection (_UpProjection, modules.py:6-31), D (modules.py:61-94), MFF (modules.py:96-128) and
 RefinementR.  In eval() every BatchNorm normalises with its running statistics and leaves them untouched; gradients
@@ -15,8 +17,8 @@ flow through it as through the frozen affine map.
 
 Activations are channels-last bf16 ([N, H, W, C], C a multiple of 64 for the convolutions, of 8 elsewhere); weights stay
 the reference's fp32 [Cout, Cin, KH, KW] parameters (state_dict compatible).  Convolutions with fewer than 64 output
-channels (the 16-channel MFF branches, the final 1-channel depth conv) are run with the output channels zero-padded to 64.
-No CPU path."""
+channels (the 16-channel MFF branches) are run with the output channels zero-padded to 64; the 1-channel depth head has
+kernels of its own (depth_head).  No CPU path."""
 import ctypes
 
 import torch
@@ -217,6 +219,47 @@ class _SplitFn(torch.autograd.Function):
         return (dy,) + (None,) * len(ctx.sizes)
 
 
+class _DepthHeadFn(torch.autograd.Function):
+    @staticmethod
+    def forward(ctx, x, weight, bias):
+        _lib.require_cuda(x, weight, bias)
+        assert x.dtype == torch.bfloat16 and x.is_contiguous() and x.dim() == 4
+        n, h, w, c = x.shape
+        assert tuple(weight.shape) == (1, c, 5, 5) and weight.dtype == torch.float32, (x.shape, weight.shape)
+        assert bias.numel() == 1 and bias.dtype == torch.float32
+        weight, bias = weight.contiguous(), bias.contiguous()
+        y = torch.empty(n, h, w, 1, dtype=torch.float32, device=x.device)
+        _lib.call("dirb200_depth_head_fwd", _lib.ptr(x), _lib.ptr(weight), _lib.ptr(bias), _lib.ptr(y), n, h, w, c,
+                  _lib.stream_ptr())
+        ctx.save_for_backward(x, weight)
+        return y
+
+    @staticmethod
+    def backward(ctx, dy):
+        x, weight = ctx.saved_tensors
+        n, h, w, c = x.shape
+        dy = dy.to(torch.float32).contiguous()
+        st = _lib.stream_ptr()
+        dx = dw = db = None
+        if ctx.needs_input_grad[0]:
+            dx = torch.empty_like(x)
+            _lib.call("dirb200_depth_head_dgrad", _lib.ptr(dy), _lib.ptr(weight), _lib.ptr(dx), n, h, w, c, st)
+        if ctx.needs_input_grad[1] or ctx.needs_input_grad[2]:
+            nbytes = _lib.raw("dirb200_depth_head_wgrad_workspace_bytes")(n, h, w, c)
+            ws = torch.empty(nbytes, dtype=torch.uint8, device=x.device)
+            dw = torch.empty(1, c, 5, 5, dtype=torch.float32, device=x.device)
+            db = torch.empty(1, dtype=torch.float32, device=x.device)
+            _lib.call("dirb200_depth_head_wgrad", _lib.ptr(x), _lib.ptr(dy), _lib.ptr(dw), _lib.ptr(db), _lib.ptr(ws),
+                      nbytes, n, h, w, c, st)
+        return dx, dw, db
+
+
+def depth_head(x, weight, bias):
+    """conv2d(x, weight, bias, stride 1, padding 2) with one output channel (R.conv2, modules.py:145, 169) for x bf16
+    [N, H, W, C] (C a multiple of 8 from 8 to 256), weight fp32 [1, C, 5, 5], bias fp32 [1] -> fp32 [N, H, W, 1]."""
+    return _DepthHeadFn.apply(x, weight, bias)
+
+
 def split_channels(y, sizes):
     """The channel ranges [0, s0), [s0, s0 + s1), ... of an NHWC bf16 tensor as contiguous tensors (channels past the
     last range are dropped; their gradient is zero)."""
@@ -407,7 +450,8 @@ def batch_norm_train(x, weight, bias, running_mean=None, running_var=None, momen
 class RefinementR(torch.nn.Module):
     """nyud2-dir/models/modules.py:128-174 (module R): conv0 5x5 -> bn0 -> relu -> conv1 5x5 -> bn1 -> relu ->
     [FDS.smooth on the 128-channel map] -> conv2 5x5 (1 channel, bias); parameter names / shapes as the reference's.
-    Input / feature maps are NHWC bf16; returns (depth [N, H, W, 1] bf16, features [N, H, W, C]) in training with FDS."""
+    Input / feature maps are NHWC bf16; the depth is fp32 [N, H, W, 1] (depth_head); returns (depth, features
+    [N, H, W, C] bf16, unsmoothed) in training with FDS."""
 
     def __init__(self, num_features=128, fds=None):
         super().__init__()
@@ -431,7 +475,7 @@ class RefinementR(torch.nn.Module):
             n, h, w, c = x1.shape
             rows = _FDS.smooth(self.FDS, x1.float().view(-1, c), depth.reshape(-1).float(), epoch)
             x1_s = rows.view(n, h, w, c).to(torch.bfloat16)
-        x2 = conv2d_nhwc(x1_s, self.conv2.weight, 1, 2) + self.conv2.bias.to(torch.bfloat16)
+        x2 = depth_head(x1_s, self.conv2.weight, self.conv2.bias)
         if self.training and self.FDS is not None:
             return x2, x1
         return x2

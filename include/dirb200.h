@@ -208,6 +208,21 @@ int dirb200_upsample_bilinear_bwd(const void* dy, int n, int h, int w, int c, in
  * NHWC tensors (modules.py:120) is one call per source; its backward is the same call with the roles swapped. */
 int dirb200_copy_channels(const void* src, int src_stride, int src_off, void* dst, int dst_stride, int dst_off, int c,
                           int64_t pixels, void* stream);
+/* The depth head of module R (modules.py:145, 169: conv2 = nn.Conv2d(c, 1, kernel_size=5, stride=1, padding=2,
+ * bias=True), x2 = conv2(x1_s)) as memory-bound kernels written for one output channel.  x bf16 NHWC [n, h, w, c];
+ * w fp32 [1, c, 5, 5] and b fp32 [1], the reference's parameters as they are.  c a multiple of 8 from 8 to 256,
+ * n, h, w > 0, n * h * w * c < 2^31.  Deterministic: every sum has a fixed order (no atomics), so repeated calls give
+ * the same bits and one image's output does not depend on the rest of the batch.
+ * fwd:   y fp32 [n, h, w, 1] (the bytes of the reference's [n, 1, h, w]) = b + sum_{ch, tap} w * x, fp32 accumulation.
+ * dgrad: dx bf16 [n, h, w, c], dx[p, ch] = sum_tap w[ch, tap] * dy[p - tap], one rounding of an fp32 sum; dy fp32.
+ * wgrad: dw fp32 [1, c, 5, 5], dw[ch, tap] = sum_p dy[p] * x[p + tap, ch], and db fp32 [1] = sum_p dy[p], both
+ *        overwritten; per-tile partials in the workspace, reduced in tile order. */
+int dirb200_depth_head_fwd(const void* x, const float* w, const float* b, float* y, int n, int h, int wd, int c,
+                           void* stream);
+int dirb200_depth_head_dgrad(const float* dy, const float* w, void* dx, int n, int h, int wd, int c, void* stream);
+size_t dirb200_depth_head_wgrad_workspace_bytes(int n, int h, int wd, int c);     /* 0 for a refused shape */
+int dirb200_depth_head_wgrad(const void* x, const float* dy, float* dw, float* db, void* workspace,
+                             size_t workspace_bytes, int n, int h, int wd, int c, void* stream);
 
 /* ------------------------------------------------ input pipeline ---- */
 /* Batched device form of the per-sample torchvision chain agedb-dir/datasets.py:38-53 after the resize:

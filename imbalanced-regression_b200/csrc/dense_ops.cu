@@ -155,8 +155,9 @@ int dirb200_upsample_bilinear_bwd(const void* dy, int n, int h, int w, int c, in
 
 int dirb200_copy_channels(const void* src, int src_stride, int src_off, void* dst, int dst_stride, int dst_off, int c,
                           int64_t pixels, void* stream) {
-  DIRB_CHECK_ARG(src && dst && c > 0 && c % 8 == 0 && src_stride % 8 == 0 && dst_stride % 8 == 0 && src_off % 8 == 0 &&
-                     dst_off % 8 == 0 && src_off + c <= src_stride && dst_off + c <= dst_stride && pixels >= 0,
+  DIRB_CHECK_ARG(src && dst && c > 0 && c % 8 == 0 && src_stride % 8 == 0 && dst_stride % 8 == 0 && src_off >= 0 &&
+                     dst_off >= 0 && src_off % 8 == 0 && dst_off % 8 == 0 && src_off + c <= src_stride &&
+                     dst_off + c <= dst_stride && pixels >= 0,
                  "copy_channels: channel counts / offsets / strides must be multiples of 8 and in range");
   if (pixels == 0) return DIRB200_OK;
   copy_channels_kernel<<<grid1d(pixels * (c / 8)), 256, 0, as_stream(stream)>>>(

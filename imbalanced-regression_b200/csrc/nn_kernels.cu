@@ -1382,7 +1382,8 @@ int dirb200_avgpool_bwd(const float* grad_out, int n, int hw, int c, void* grad_
 
 int dirb200_linear1_fwd(const float* x, const float* w, const float* bias, int64_t n, int d, float* pred,
                         void* stream) {
-  DIRB_CHECK_ARG(x && w && bias && pred && n > 0 && d > 0, "linear1_fwd: bad arguments");
+  // one CTA per row: n is the grid size
+  DIRB_CHECK_ARG(x && w && bias && pred && n > 0 && n <= INT32_MAX && d > 0, "linear1_fwd: bad arguments");
   linear1_fwd_kernel<<<(unsigned)n, 256, 0, as_stream(stream)>>>(x, w, bias, d, pred);
   DIRB_LAUNCHED();
   return DIRB200_OK;
@@ -1390,7 +1391,8 @@ int dirb200_linear1_fwd(const float* x, const float* w, const float* bias, int64
 
 int dirb200_linear1_bwd(const float* grad_pred, const float* x, const float* w, int64_t n, int d, float* dx,
                         float* dw, float* dbias, void* stream) {
-  DIRB_CHECK_ARG(grad_pred && x && w && dw && dbias && n > 0 && d > 0, "linear1_bwd: bad arguments");
+  // the kernel walks the n rows with a 32-bit counter
+  DIRB_CHECK_ARG(grad_pred && x && w && dw && dbias && n > 0 && n <= INT32_MAX && d > 0, "linear1_bwd: bad arguments");
   linear1_bwd_kernel<<<(d + 127) / 128, 128, 0, as_stream(stream)>>>(grad_pred, x, w, (int)n, d, dx, dw, dbias);
   DIRB_LAUNCHED();
   return DIRB200_OK;

@@ -83,6 +83,9 @@ _SIGS = {
     "dirb200_depth_head_wgrad_workspace_bytes": (c_size_t, [c_int, c_int, c_int, c_int]),
     "dirb200_depth_head_wgrad": (c_int, [P, P, P, P, P, c_size_t, c_int, c_int, c_int, c_int, P]),
     "dirb200_augment_batch": (c_int, [P, P, P, c_int, c_int, c_int, c_float, c_float, P, P]),
+    "dirb200_depth_augment_workspace_bytes": (c_size_t, [c_int, c_int, c_int, c_int, c_int]),
+    "dirb200_depth_augment_batch": (c_int, [P, P, c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_int, P, P, P, P,
+                                            P, P, P, c_int, P, P, P, P, P, P, c_size_t, P]),
 }
 
 

@@ -233,6 +233,33 @@ int dirb200_depth_head_wgrad(const void* x, const float* dy, float* dw, float* d
 int dirb200_augment_batch(const uint8_t* images, const int* crop_yx, const uint8_t* flip, int n, int size, int pad,
                           float mean, float stdv, float* out, void* stream);
 
+/* Batched device form of NYUD2-DIR's per-sample chains after Scale(240) (nyud2-dir/loaddata.py:108-125 training,
+ * :132-148 FDS, :151-170 test, with nyud2-dir/nyu_transform.py), plus _get_weights (loaddata.py:58-67).
+ * images u8 [n][h][w][3] (RGB, HWC); depths u8 [n][h][w] (depth_u16 = 0) or u16 [n][h][w] (depth_u16 = 1: the test
+ * chain, int16 / 1000, no flip / rotation / resize).  Outputs: image_out f32 [n][3][crop_h][crop_w], depth_out and
+ * weight_out f32 [n][1][depth_h][depth_w] (weight_out may be NULL without a table).
+ *   flip u8 [n] (NULL: none): RandomHorizontalFlip, before the rotation (nyu_transform.py:55-71);
+ *   affine f64 [n][6] = (m00, m01, m10, m11, offset0, offset1) of scipy.ndimage.rotate(reshape=False) over the
+ *     (h, w) plane (NULL: no rotation): RandomRotate(5), order-2 spline, mode 'constant' (:24-53), bit-exact uint8;
+ *   CenterCrop at (round((w - crop_w) / 2), round((h - crop_h) / 2)), half to even; the depth crop resized to
+ *     depth_h x depth_w by Pillow's 8-bit BICUBIC (:118-148), bit-exact; ToTensor: u8 / 255, depth * 10 (:151-213);
+ *   rgb_offset f32 [n][3] (NULL: none): Lighting's per-channel offset (:216-236), computed on the host;
+ *   jitter_order i32 [n][3] (0 brightness, 1 contrast, 2 saturation) and jitter_alpha f32 [n][3], the weight of the
+ *     k-th applied transform (NULL, NULL: none): ColorJitter (:239-312); Contrast's mean is reduced in fp64;
+ *   mean_std: HOST f32 [6], Normalize's mean then std (:315-347);
+ *   bucket_weights f32 [n_buckets >= 100] on the device: weight = table[min(int(depth * 10), 99)] (NULL: ones).
+ * debug_crop u8 [n][crop_h][crop_w][4] (R, G, B, depth after flip + rotation + crop) and debug_mean f32 [n] (Contrast's
+ * grayscale mean; written only with jitter): optional test outputs, NULL to skip.
+ * Every argument is checked before any CUDA call. */
+size_t dirb200_depth_augment_workspace_bytes(int n, int h, int w, int crop_h, int crop_w);
+int dirb200_depth_augment_batch(const uint8_t* images, const void* depths, int depth_u16, int n, int h, int w,
+                                int crop_h, int crop_w, int depth_h, int depth_w, const uint8_t* flip,
+                                const double* affine, const float* rgb_offset, const int* jitter_order,
+                                const float* jitter_alpha, const float* mean_std, const float* bucket_weights,
+                                int n_buckets, float* image_out, float* depth_out, float* weight_out,
+                                uint8_t* debug_crop, float* debug_mean, void* workspace, size_t workspace_bytes,
+                                void* stream);
+
 /* ------------------------------------------------ evaluation metrics ---- */
 /* hist[int(label)] += 1 for 0 <= int(label) < nbins (int64, bit-exact, ADDS; no clamping): the per-label-value
  * training counts that shot_metrics compares against, agedb-dir/train.py:339,350. */

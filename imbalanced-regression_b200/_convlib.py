@@ -14,10 +14,6 @@ _lib.register({
     "dirb200_conv_wgrad_workspace_bytes": (c_size_t, _I9 + [c_int]),
     "dirb200_conv_wgrad": (c_int, [P, P, P, P, c_size_t] + _I9 + [c_int, c_int, P]),
     "dirb200_conv_plan": (c_int, _I9 + [c_int, c_int, P]),
-    # 5x5 convolutions over an up-sampled operand (the _UpProjection of NYUD2-DIR's D / MFF)
-    "dirb200_conv_fprop_upsampled": (c_int, [P, P, P] + [c_int] * 7 + [P]),
-    "dirb200_conv_wgrad_upsampled_workspace_bytes": (c_size_t, [c_int] * 7),
-    "dirb200_conv_wgrad_upsampled": (c_int, [P, P, P, P, c_size_t] + [c_int] * 8 + [P]),
     "dirb200_bn_eval_coeffs": (c_int, [c_int, P, P, c_float, P, P, P, P, P]),
     # test aids: the fused BatchNorm epilogues and their consumers
     "dirb200_conv_fprop_bn_stats": (c_int, [P, P, P] + _I9 + [c_int, P, P, P]),

@@ -50,14 +50,6 @@ int conv_wgrad_partials(const __nv_bfloat16* x, const __nv_bfloat16* dy, float* 
                         int* splits_out, cudaStream_t st);
 int wgrad_reduce(const float* workspace, int splits, float* dw, const ConvShape& s, bool stem, bool accumulate,
                  cudaStream_t st);
-// 5x5 / stride-1 / pad-2 convolutions over F.upsample(x, (ho, wo), bilinear) of x [n][h][w][cin], the up-sampled
-// operand formed in the producer warps and never stored (conv_igemm.cu); check_upsampled_conv: host-only argument check
-int check_upsampled_conv(int n, int h, int w, int cin, int cout, int ho, int wo, const char* who);
-int conv_fprop_upsampled(const __nv_bfloat16* x, const __nv_bfloat16* w_fprop, __nv_bfloat16* y, int n, int h, int w,
-                         int cin, int cout, int ho, int wo, cudaStream_t st);
-size_t conv_wgrad_upsampled_workspace_bytes(int n, int cin, int cout, int ho, int wo);
-int conv_wgrad_partials_upsampled(const __nv_bfloat16* x, const __nv_bfloat16* dy, float* partial, int n, int h, int w,
-                                  int cin, int cout, int ho, int wo, int* splits_out, cudaStream_t st);
 int conv_wgrad(const __nv_bfloat16* x, const __nv_bfloat16* dy, float* dw, float* workspace, const ConvShape& s,
                bool stem, bool accumulate, cudaStream_t st);
 struct WgradReduceDesc {        // one conv layer's split-K reduction job (see wgrad_reduce_all)

@@ -309,38 +309,6 @@ int dirb200_conv_wgrad(const void* x, const void* dy, float* dw, void* workspace
                     accumulate != 0, as_stream(stream));
 }
 
-/* ---- Convolutions over an up-sampled operand (see include/dirb200.h). */
-int dirb200_conv_fprop_upsampled(const void* x, const void* w_fprop, void* y, int n, int h, int w, int cin, int cout,
-                                 int ho, int wo, void* stream) {
-  DIRB_CHECK_ARG(x && w_fprop && y, "conv_fprop_upsampled: null pointer");
-  return conv_fprop_upsampled((const __nv_bfloat16*)x, (const __nv_bfloat16*)w_fprop, (__nv_bfloat16*)y, n, h, w, cin,
-                              cout, ho, wo, as_stream(stream));
-}
-
-size_t dirb200_conv_wgrad_upsampled_workspace_bytes(int n, int h, int w, int cin, int cout, int ho, int wo) {
-  if (check_upsampled_conv(n, h, w, cin, cout, ho, wo, "conv_wgrad_upsampled_workspace_bytes")) return 0;
-  return conv_wgrad_upsampled_workspace_bytes(n, cin, cout, ho, wo);
-}
-
-int dirb200_conv_wgrad_upsampled(const void* x, const void* dy, float* dw, void* workspace, size_t workspace_bytes, int n,
-                                 int h, int w, int cin, int cout, int ho, int wo, int accumulate, void* stream) {
-  DIRB_CHECK_ARG(x && dy && dw && workspace, "conv_wgrad_upsampled: null pointer");
-  // every argument before the workspace size (which asks the device for its SM count)
-  if (int rc = check_upsampled_conv(n, h, w, cin, cout, ho, wo, "conv_wgrad_upsampled")) return rc;
-  const size_t need = conv_wgrad_upsampled_workspace_bytes(n, cin, cout, ho, wo);
-  if (workspace_bytes < need) {
-    set_error("conv_wgrad_upsampled: workspace too small (%zu < %zu)", workspace_bytes, need);
-    return DIRB200_ERR_WORKSPACE;
-  }
-  cudaStream_t st = as_stream(stream);
-  int splits = 1;
-  if (int rc = conv_wgrad_partials_upsampled((const __nv_bfloat16*)x, (const __nv_bfloat16*)dy, (float*)workspace, n, h,
-                                             w, cin, cout, ho, wo, &splits, st))
-    return rc;
-  const ConvShape s{n, ho, wo, cin, cout, 5, 5, 1, 2, ho, wo};
-  return wgrad_reduce((const float*)workspace, splits, dw, s, false, accumulate != 0, st);
-}
-
 /* ---- Test aids: the fused epilogues the network runner uses, one call each (see include/dirb200.h). */
 static void layout_to_host(const StatLayout& l, int* layout_host) {
   layout_host[0] = l.rows; layout_host[1] = l.n_tiles; layout_host[2] = l.bn; layout_host[3] = l.group;

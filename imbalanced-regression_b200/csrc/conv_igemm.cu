@@ -14,7 +14,6 @@
 #include "common.cuh"
 #include "tc.cuh"
 #include "conv.cuh"
-#include "upsample.cuh"
 
 namespace dirb200 {
 using namespace tc;
@@ -72,11 +71,6 @@ struct IgemmParams {
   const __nv_bfloat16* bst_y;
   const float* bst_scale;
   const float* bst_shift;
-  // UPS kernels (5x5 / stride-1 convolutions over F.upsample(x, (hs, ws), bilinear), nyud2-dir/models/modules.py:23-27):
-  // the gathered tensor (hs x ws, cs channels) is never stored; src is the low-resolution x [n][up_h][up_w][cs] and
-  // every A row is interpolated from it (up_sh / up_sw = up_h / hs, up_w / ws as float, as the standalone kernel's)
-  int up_h, up_w;
-  float up_sh, up_sw;
 };
 
 template <int BN, bool STAGED_EPI>
@@ -161,47 +155,11 @@ __device__ __forceinline__ const __nv_bfloat16* tap_source(const IgemmParams& P,
   return ok ? P.src + (static_cast<size_t>(rp.nb + hi) * P.ws + wi) * P.cs + coff : P.src;
 }
 
-// UPS: the 16 bytes at channel offset `coff` of pixel (y - pad + r, x - pad + s) of up = F.upsample(src, (hs, ws)) for
-// the packed GEMM-row pixel pk (zeros outside the up-sampled image or past the last row): the four source pixels,
-// interpolated in fp32 with upsample.cuh's arithmetic and rounded to bf16 -- dirb200_upsample_bilinear_fwd's values.
-__device__ __forceinline__ uint4 upsampled_16b(const IgemmParams& P, uint32_t pk, int r, int s, int coff) {
-  const int n = (pk >> 18) & 0x1FFF;
-  const int uy = static_cast<int>((pk >> 9) & 0x1FF) - P.pad + r, ux = static_cast<int>(pk & 0x1FF) - P.pad + s;
-  uint4 out = make_uint4(0u, 0u, 0u, 0u);
-  if ((pk >> 31) && static_cast<unsigned>(uy) < static_cast<unsigned>(P.hs) &&
-      static_cast<unsigned>(ux) < static_cast<unsigned>(P.ws)) {
-    int y0, y1, x0, x1;
-    float ly, lx;
-    upsample_src_index(uy, P.up_sh, P.up_h, y0, y1, ly);
-    upsample_src_index(ux, P.up_sw, P.up_w, x0, x1, lx);
-    const __nv_bfloat16* base = P.src + static_cast<size_t>(n) * P.up_h * P.up_w * P.cs + coff;
-    const uint4 a00 = __ldg(reinterpret_cast<const uint4*>(base + (static_cast<size_t>(y0) * P.up_w + x0) * P.cs));
-    const uint4 a01 = __ldg(reinterpret_cast<const uint4*>(base + (static_cast<size_t>(y0) * P.up_w + x1) * P.cs));
-    const uint4 a10 = __ldg(reinterpret_cast<const uint4*>(base + (static_cast<size_t>(y1) * P.up_w + x0) * P.cs));
-    const uint4 a11 = __ldg(reinterpret_cast<const uint4*>(base + (static_cast<size_t>(y1) * P.up_w + x1) * P.cs));
-    const float hy = __fsub_rn(1.f, ly), hx = __fsub_rn(1.f, lx);
-    const uint32_t w00[4] = {a00.x, a00.y, a00.z, a00.w}, w01[4] = {a01.x, a01.y, a01.z, a01.w};
-    const uint32_t w10[4] = {a10.x, a10.y, a10.z, a10.w}, w11[4] = {a11.x, a11.y, a11.z, a11.w};
-    uint32_t o[4];
-#pragma unroll
-    for (int e = 0; e < 4; ++e) {
-      const float lo = upsample_lerp(__uint_as_float(w00[e] << 16), __uint_as_float(w01[e] << 16),
-                                     __uint_as_float(w10[e] << 16), __uint_as_float(w11[e] << 16), hx, lx, hy, ly);
-      const float hi = upsample_lerp(__uint_as_float(w00[e] & 0xffff0000u), __uint_as_float(w01[e] & 0xffff0000u),
-                                     __uint_as_float(w10[e] & 0xffff0000u), __uint_as_float(w11[e] & 0xffff0000u), hx,
-                                     lx, hy, ly);
-      __nv_bfloat162 h = __floats2bfloat162_rn(lo, hi);
-      o[e] = *reinterpret_cast<uint32_t*>(&h);
-    }
-    out = make_uint4(o[0], o[1], o[2], o[3]);
-  }
-  return out;
-}
 // ATMA: the A operand comes by TMA -- tiled maps for 1x1 / stride-1 convolutions (a plain [pixels][channels] matrix:
 // K-major 64 x 128 boxes for fprop / dgrad, two 64 x 64 MN-major boxes for wgrad), im2col-mode maps for the 3x3 and
 // strided ones -- issued by warp 0.  Without ATMA (stem, or with the TMA forms switched off) warps 0-3 gather the rows
-// with cp.async.  UPS: warps 0-3 compute the A rows from a low-resolution source (upsampled_16b) and store them.
-template <int BN, bool WGRAD, bool STEM, bool ATMA = false, bool AFFINE = false, bool BSTAT = false, bool UPS = false>
+// with cp.async.
+template <int BN, bool WGRAD, bool STEM, bool ATMA = false, bool AFFINE = false, bool BSTAT = false>
 __global__ void __launch_bounds__(kThreads, 1)
 igemm_kernel(const __grid_constant__ CUtensorMap tmap_b, const __grid_constant__ CUtensorMap tmap_a,
              const IgemmParams P) {
@@ -211,7 +169,6 @@ igemm_kernel(const __grid_constant__ CUtensorMap tmap_b, const __grid_constant__
   // the folded-BN epilogue reads only the accumulators and P: it does not depend on how the A operand arrived
   static_assert(!AFFINE || (!WGRAD && !STEM), "folded-BN epilogue: non-stem fprop GEMMs only");
   static_assert(!BSTAT || (ATMA && !WGRAD && !AFFINE), "BN-backward moments in the epilogue: TMA-fed dgrad GEMMs only");
-  static_assert(!UPS || (!ATMA && !STEM && !AFFINE && !BSTAT), "up-sampled A operand: plain fprop / wgrad GEMMs only");
   extern __shared__ uint8_t smem_raw[];
   const uint32_t smem_base = (smem_u32(smem_raw) + 1023u) & ~1023u;
   uint8_t* const smem_gen = smem_raw + (smem_base - smem_u32(smem_raw));
@@ -270,87 +227,7 @@ igemm_kernel(const __grid_constant__ CUtensorMap tmap_b, const __grid_constant__
   __syncthreads();
 
   if (warp < 4) {
-    if constexpr (UPS) {
-      // ===== A computed from the low-resolution source (4 warps) + B by TMA (warp 0) =====
-      // Same row / column assignment and swizzled slots as the cp.async gather below: a thread serves 8 rows, always
-      // the same 16-byte column j.  fprop rows are fixed per tile (packed pixels resolved once); wgrad rows are the
-      // k-block's pixels for the warp's fixed (tap, 64-channel chunk), one packed pixel per lane, fetched by shuffle.
-      // Generic-proxy stores: fence.proxy.async, then one mbarrier arrival per thread (the consumers fence as well).
-      const int j = lane & 7;
-      const int q = lane >> 3;
-      uint32_t rs = 0, rph = 0;
-      for (int t = tile_first; t < tile_end; t += tile_step) {
-        int split, m_tile, n_tile, kb_begin, nk;
-        decode_tile(t, split, m_tile, n_tile, kb_begin, nk);
-        const int n0 = n_tile * BN;
-        uint32_t pk8[8];
-        int chunk_r = 0, chunk_s = 0, chunk_c0 = 0;
-        bool chunk_ok = true;
-        uint32_t tile_off;
-        if constexpr (!WGRAD) {
-          const uint32_t mypk = pack_pixel(static_cast<long long>(m_tile) * BM + warp * 32 + lane, P);
-#pragma unroll
-          for (int i = 0; i < 8; ++i) pk8[i] = __shfl_sync(0xffffffffu, mypk, 4 * i + q);
-          tile_off = warp * 32 * 128;
-        } else {
-          const int chunk = warp >> 1;
-          const int gchunk = m_tile * 2 + chunk;
-          chunk_ok = gchunk < P.total_chunks;
-          uint32_t tap, cbk, cr, csx;
-          P.fd_cpb.divmod(static_cast<uint32_t>(gchunk), tap, cbk);
-          P.fd_kw.divmod(tap, cr, csx);
-          chunk_c0 = static_cast<int>(cbk) * 64;
-          chunk_r = static_cast<int>(cr);
-          chunk_s = static_cast<int>(csx);
-          tile_off = chunk * 8192 + (warp & 1) * 32 * 128;
-        }
-        int tc = 0, cb = 0;
-        for (int it = 0; it < nk; ++it) {
-          const int s = static_cast<int>(rs);
-          mbar_wait(empty_bar(s), rph ^ 1u);
-          if (++rs == nstages) { rs = 0; rph ^= 1u; }
-          const int kb = kb_begin + it;
-          const uint32_t dst_base = a_addr(s) + tile_off;
-          int kcoord = kb, r, sx, coff;
-          uint32_t mypk = 0u;
-          if constexpr (!WGRAD) {
-            r = P.tap_r[tc];
-            sx = P.tap_s[tc];
-            coff = cb * 64 + j * 8;
-            kcoord = P.tap_list[tc] * P.cpb + cb;
-            if (++cb == P.cpb) { cb = 0; ++tc; }
-          } else {
-            r = chunk_r;
-            sx = chunk_s;
-            coff = chunk_c0 + j * 8;
-            mypk = chunk_ok ? pack_pixel(static_cast<long long>(kb) * 64 + (warp & 1) * 32 + lane, P) : 0u;
-          }
-#pragma unroll
-          for (int i = 0; i < 8; ++i) {
-            const int row = 4 * i + q;
-            const uint32_t pk = WGRAD ? __shfl_sync(0xffffffffu, mypk, row) : pk8[i];
-            const uint4 v = upsampled_16b(P, pk, r, sx, coff);
-            asm volatile("st.shared.v4.b32 [%0], {%1, %2, %3, %4};" ::"r"(dst_base + row * 128 + ((j ^ (row & 7)) << 4)),
-                         "r"(v.x), "r"(v.y), "r"(v.z), "r"(v.w) : "memory");
-          }
-          if (warp == 0) {
-            if (elect_one()) {
-              mbar_arrive_expect_tx(full_bar(s), C::kBBytes);
-              if constexpr (!WGRAD) {
-                tma_load_2d(b_addr(s), &tmap_b, full_bar(s), kcoord * BK, n0);
-              } else {
-#pragma unroll
-                for (int i = 0; i < BN / 64; ++i)
-                  tma_load_2d(b_addr(s) + i * 8192, &tmap_b, full_bar(s), n0 + 64 * i, kb * 64);
-              }
-            }
-            __syncwarp();
-          }
-          fence_proxy_async();
-          mbar_arrive(full_bar(s));
-        }
-      }
-    } else if constexpr (!ATMA) {
+    if constexpr (!ATMA) {
       // ===== A producer (4 warps) + B by TMA (warp 0) =====
       // Address generation is hoisted out of the k-loop: per tile each thread precomputes, for its 8 rows, the
       // element offset of the filter-tap origin and a bit mask of the taps that fall inside the image; per k-block
@@ -887,13 +764,13 @@ static IgemmParams finish_params(const IgemmParams& P) {
   return Q;
 }
 
-template <int BN, bool WGRAD, bool STEM, bool ATMA = false, bool AFFINE = false, bool BSTAT = false, bool UPS = false>
+template <int BN, bool WGRAD, bool STEM, bool ATMA = false, bool AFFINE = false, bool BSTAT = false>
 static int launch_igemm_impl(const CUtensorMap& tm, const CUtensorMap& tma, const IgemmParams& Qin, cudaStream_t st) {
   using C = Cfg<BN, !WGRAD>;
   const IgemmParams Q = finish_params(Qin);
   static bool configured = false;
   if (!configured) {
-    DIRB_CUDA(cudaFuncSetAttribute(igemm_kernel<BN, WGRAD, STEM, ATMA, AFFINE, BSTAT, UPS>,
+    DIRB_CUDA(cudaFuncSetAttribute(igemm_kernel<BN, WGRAD, STEM, ATMA, AFFINE, BSTAT>,
                                    cudaFuncAttributeMaxDynamicSharedMemorySize, C::kSmemBytes));
     configured = true;
   }
@@ -902,7 +779,7 @@ static int launch_igemm_impl(const CUtensorMap& tm, const CUtensorMap& tma, cons
   // below the tile count (the extra CTAs run as a second wave)
   if (!WGRAD && grid < Q.n_tiles) grid = Q.n_tiles;
   t_last_layout = StatLayout{grid, Q.n_tiles, BN, 1};
-  igemm_kernel<BN, WGRAD, STEM, ATMA, AFFINE, BSTAT, UPS><<<grid, kThreads, C::kSmemBytes, st>>>(tm, tma, Q);
+  igemm_kernel<BN, WGRAD, STEM, ATMA, AFFINE, BSTAT><<<grid, kThreads, C::kSmemBytes, st>>>(tm, tma, Q);
   DIRB_LAUNCHED();
   return DIRB200_OK;
 }
@@ -1211,91 +1088,6 @@ int conv_wgrad_partials(const __nv_bfloat16* x, const __nv_bfloat16* dy, float* 
     return DISPATCH_BN(bn, true, false, tm, P, m_tiles, splits, st, &ta);
   }
   return DISPATCH_BN(bn, true, false, tm, P, m_tiles, splits, st);
-}
-
-// ---- 5x5 / stride-1 / pad-2 convolutions over up = F.upsample(x, (ho, wo), bilinear)  (nyud2-dir/models/modules.py:23-27)
-// The A operand is interpolated from x by the UPS producer; tile width, tile walk and split-K plan are those of
-// conv_fprop / conv_wgrad on the stored up, so each result equals that composition to the bit.
-int check_upsampled_conv(int n, int h, int w, int cin, int cout, int ho, int wo, const char* who) {
-  DIRB_CHECK_ARG(n > 0 && h > 0 && w > 0 && ho > 0 && wo > 0, "%s: sizes must be positive", who);
-  DIRB_CHECK_ARG(ho >= h && wo >= w, "%s: the target size must be at least the source size (%dx%d -> %dx%d)", who, h, w,
-                 ho, wo);
-  DIRB_CHECK_ARG(cin > 0 && cin % 64 == 0, "%s: Cin must be a positive multiple of 64 (got %d)", who, cin);
-  DIRB_CHECK_ARG(cout > 0 && cout % 64 == 0, "%s: Cout must be a positive multiple of 64 (got %d)", who, cout);
-  // packed GEMM-row pixel: 13-bit image, 9-bit row and column of the up-sampled (= output) grid
-  DIRB_CHECK_ARG(n <= 8192 && ho <= 512 && wo <= 512, "%s: at most 8192 images of at most 512 x 512 (got %d x %dx%d)",
-                 who, n, ho, wo);
-  DIRB_CHECK_ARG(static_cast<long long>(n) * ho * wo < (1LL << 31), "%s: more than 2^31 pixels", who);
-  return DIRB200_OK;
-}
-
-static ConvShape upsampled_shape(int n, int cin, int cout, int ho, int wo) {
-  return ConvShape{n, ho, wo, cin, cout, 5, 5, 1, 2, ho, wo};
-}
-
-static IgemmParams upsampled_params(const __nv_bfloat16* x, int n, int h, int w, int cin, int ho, int wo) {
-  IgemmParams P{};
-  P.src = x; P.n = n; P.hs = ho; P.ws = wo; P.cs = cin; P.hm = ho; P.wm = wo;
-  P.kh = 5; P.kw = 5; P.stride = 1; P.pad = 2; P.transposed = 0;
-  P.cpb = cin / 64;
-  P.pixels = static_cast<long long>(n) * ho * wo;
-  P.ntaps_c = 25;
-  for (int i = 0; i < kMaxTaps; ++i) P.tap_list[i] = i;
-  P.up_h = h; P.up_w = w;
-  P.up_sh = static_cast<float>(h) / ho;      // the scales dirb200_upsample_bilinear_fwd passes
-  P.up_sw = static_cast<float>(w) / wo;
-  return P;
-}
-
-template <int BN, bool WGRAD>
-static int launch_upsampled(const CUtensorMap& tm, const IgemmParams& P, int m_tiles, int splits, cudaStream_t st) {
-  IgemmParams Q = P;
-  Q.m_tiles = m_tiles;
-  Q.num_tiles = m_tiles * P.n_tiles * splits;
-  return launch_igemm_impl<BN, WGRAD, false, false, false, false, true>(tm, tm, Q, st);
-}
-
-int conv_fprop_upsampled(const __nv_bfloat16* x, const __nv_bfloat16* w_fprop, __nv_bfloat16* y, int n, int h, int w,
-                         int cin, int cout, int ho, int wo, cudaStream_t st) {
-  if (int rc = check_upsampled_conv(n, h, w, cin, cout, ho, wo, "conv_fprop_upsampled")) return rc;
-  const ConvShape s = upsampled_shape(n, cin, cout, ho, wo);
-  if (int rc = check_shape(s, false, "conv_fprop_upsampled")) return rc;
-  const int ktot = 25 * cin;
-  IgemmParams P = upsampled_params(x, n, h, w, cin, ho, wo);
-  P.num_kblocks = ktot / 64;
-  P.ldc = cout; P.out = y;
-  const int m_tiles = static_cast<int>((P.pixels + BM - 1) / BM);
-  const int bn = pick_bn(cout);
-  P.n_tiles = cout / bn;
-  CUtensorMap tm;
-  if (int rc = make_tmap_bf16_2d(&tm, w_fprop, ktot, cout, static_cast<uint64_t>(ktot) * 2, bn)) return rc;
-  return bn == 128 ? launch_upsampled<128, false>(tm, P, m_tiles, 1, st) : launch_upsampled<64, false>(tm, P, m_tiles, 1, st);
-}
-
-size_t conv_wgrad_upsampled_workspace_bytes(int n, int cin, int cout, int ho, int wo) {
-  return conv_wgrad_workspace_bytes(upsampled_shape(n, cin, cout, ho, wo));
-}
-
-int conv_wgrad_partials_upsampled(const __nv_bfloat16* x, const __nv_bfloat16* dy, float* partial, int n, int h, int w,
-                                  int cin, int cout, int ho, int wo, int* splits_out, cudaStream_t st) {
-  if (int rc = check_upsampled_conv(n, h, w, cin, cout, ho, wo, "conv_wgrad_upsampled")) return rc;
-  const ConvShape s = upsampled_shape(n, cin, cout, ho, wo);
-  if (int rc = check_shape(s, false, "conv_wgrad_upsampled")) return rc;
-  IgemmParams P = upsampled_params(x, n, h, w, cin, ho, wo);
-  P.num_kblocks = static_cast<int>((P.pixels + 63) / 64);
-  P.total_chunks = 25 * cin / 64;
-  const int splits = conv_wgrad_splits(s);
-  P.kblocks_per_split = (P.num_kblocks + splits - 1) / splits;
-  P.ldc = cout; P.out = partial;
-  const int bn = wgrad_bn(s);
-  P.n_tiles = cout / bn;
-  const int m_tiles = (P.total_chunks + 1) / 2;
-  *splits_out = splits;
-  CUtensorMap tm;
-  if (int rc = make_tmap_bf16_2d(&tm, dy, cout, static_cast<uint64_t>(P.pixels), static_cast<uint64_t>(cout) * 2, 64))
-    return rc;
-  return bn == 128 ? launch_upsampled<128, true>(tm, P, m_tiles, splits, st)
-                   : launch_upsampled<64, true>(tm, P, m_tiles, splits, st);
 }
 
 // Host-only description of the launch a conv would get (no CUDA call): which tile width, operand feeding form and

@@ -6,8 +6,6 @@
   upsample_bilinear(x, size)                F.upsample(x, size=size, mode='bilinear') (modules.py:24)
   cat_channels(tensors)                     torch.cat(tensors, 1) (modules.py:120)
   batch_norm_train(x, weight, bias, ...)    nn.BatchNorm2d in training mode [+ ReLU] (modules.py:13-21, 65, 109, 137-141)
-  conv5x5_upsampled(x, weight, size)        conv(F.upsample(x, size), weight), 5x5 / stride 1 / pad 2 (modules.py:24-27):
-                                            the up-sampled operand is formed inside the conv and never stored
   depth_head(x, weight, bias)               R's 1-channel 5x5 conv2 with bias (modules.py:145, 169): its own memory-bound
                                             kernels, fp32 output
 
@@ -137,55 +135,6 @@ class _CatFn(torch.autograd.Function):
 def cat_channels(tensors):
     """torch.cat(tensors, 1) for NHWC bf16 tensors (channel counts multiples of 8)."""
     return _CatFn.apply(*tensors)
-
-
-class _UpConvFn(torch.autograd.Function):
-    @staticmethod
-    def forward(ctx, x, weight, ho, wo):
-        _lib.require_cuda(x, weight)
-        assert x.dtype == torch.bfloat16 and x.is_contiguous() and weight.dtype == torch.float32
-        n, h, w, cin = x.shape
-        cout, cin_w, kh, kw = weight.shape
-        assert cin == cin_w and kh == kw == 5, (x.shape, weight.shape)
-        st = _lib.stream_ptr()
-        wf = torch.empty(cout, 5, 5, cin, dtype=torch.bfloat16, device=x.device)
-        wd = torch.empty(cin, 5, 5, cout, dtype=torch.bfloat16, device=x.device)
-        _lib.call("dirb200_conv_prep_weights", _lib.ptr(weight.contiguous()), cout, cin, 5, 5, 0, _lib.ptr(wf), _lib.ptr(wd), st)
-        y = torch.empty(n, ho, wo, cout, dtype=torch.bfloat16, device=x.device)
-        _lib.call("dirb200_conv_fprop_upsampled", _lib.ptr(x), _lib.ptr(wf), _lib.ptr(y), n, h, w, cin, cout, ho, wo, st)
-        ctx.save_for_backward(x, wd)         # x at input resolution: the wgrad interpolates it again
-        ctx.dims = (n, h, w, cin, cout, ho, wo)
-        return y
-
-    @staticmethod
-    def backward(ctx, dy):
-        x, wd = ctx.saved_tensors
-        n, h, w, cin, cout, ho, wo = ctx.dims
-        dy = dy.contiguous()
-        st = _lib.stream_ptr()
-        dx = dw = None
-        if ctx.needs_input_grad[0]:
-            dup = torch.empty(n, ho, wo, cin, dtype=torch.bfloat16, device=x.device)
-            _lib.call("dirb200_conv_dgrad", _lib.ptr(dy), _lib.ptr(wd), _lib.ptr(dup), n, ho, wo, cin, cout, 5, 5, 1, 2, st)
-            dx = torch.empty_like(x)
-            _lib.call("dirb200_upsample_bilinear_bwd", _lib.ptr(dup), n, h, w, cin, ho, wo, _lib.ptr(dx), st)
-        if ctx.needs_input_grad[1]:
-            nbytes = _lib.raw("dirb200_conv_wgrad_upsampled_workspace_bytes")(n, h, w, cin, cout, ho, wo)
-            ws = torch.empty(nbytes, dtype=torch.uint8, device=x.device)
-            dw = torch.empty(cout, cin, 5, 5, dtype=torch.float32, device=x.device)
-            _lib.call("dirb200_conv_wgrad_upsampled", _lib.ptr(x), _lib.ptr(dy), _lib.ptr(dw), _lib.ptr(ws), nbytes,
-                      n, h, w, cin, cout, ho, wo, 0, st)
-        return dx, dw, None, None
-
-
-def conv5x5_upsampled(x, weight, size):
-    """conv2d(F.upsample(x, size, mode='bilinear'), weight, stride 1, padding 2) for x bf16 [N, H, W, Cin] (Cin a
-    multiple of 64) and weight fp32 [Cout, Cin, 5, 5] -> bf16 [N, Ho, Wo, Cout'] with Cout' = Cout rounded up to a
-    multiple of 64 (the extra channels are zeros).  Bit-identical to conv2d_nhwc(upsample_bilinear(x, size), ...)."""
-    cout = weight.shape[0]
-    if cout % 64 != 0:
-        weight = torch.cat([weight, weight.new_zeros(64 - cout % 64, *weight.shape[1:])], 0)
-    return _UpConvFn.apply(x, weight, int(size[0]), int(size[1]))
 
 
 class _SplitFn(torch.autograd.Function):
@@ -490,12 +439,10 @@ class UpProjection(torch.nn.Module):
     conv1(x))))) + bn2(conv2(x))).  Parameter names / shapes (state_dict keys) as the reference's.
 
     conv1 and conv2 read the same up-sampled x: they run as ONE convolution with their weights concatenated along Cout,
-    and the result is split by channel (branch_convs).  By default the up-sampled x is stored (upsample_bilinear) and
-    convolved; with fused_upsample=True the convolution forms it in its producer warps and it is never stored
-    (conv5x5_upsampled: the same bits, a fraction of the memory at output resolution, but slower).  With Cout = 16
-    (MFF) conv1_2 (16 -> 16, 3x3) runs with its input channels zero-padded to 64 (conv1_2_nhwc)."""
+    and the result is split by channel (branch_convs).  With Cout = 16 (MFF) conv1_2 (16 -> 16, 3x3) runs with its
+    input channels zero-padded to 64 (conv1_2_nhwc)."""
 
-    def __init__(self, num_input_features, num_output_features, fused_upsample=False):
+    def __init__(self, num_input_features, num_output_features):
         super().__init__()
         nn = torch.nn
         self.conv1 = nn.Conv2d(num_input_features, num_output_features, kernel_size=5, stride=1, padding=2, bias=False)
@@ -506,18 +453,14 @@ class UpProjection(torch.nn.Module):
         self.bn1_2 = nn.BatchNorm2d(num_output_features)
         self.conv2 = nn.Conv2d(num_input_features, num_output_features, kernel_size=5, stride=1, padding=2, bias=False)
         self.bn2 = nn.BatchNorm2d(num_output_features)
-        self.fused_upsample = fused_upsample
 
     def branch_convs(self, x, size):
         """(conv1(up), conv2(up)) for up = F.upsample(x, size): one paired convolution, split by channel."""
         c = self.conv1.out_channels
         w = torch.cat([self.conv1.weight, self.conv2.weight], 0)
-        if self.fused_upsample:
-            y = conv5x5_upsampled(x, w, size)
-        else:
-            if w.shape[0] % 64 != 0:                  # zero-padded output channels, dropped by the split
-                w = torch.cat([w, w.new_zeros(64 - w.shape[0] % 64, *w.shape[1:])], 0)
-            y = _ConvFn.apply(upsample_bilinear(x, size), w, 1, 2)
+        if w.shape[0] % 64 != 0:                      # zero-padded output channels, dropped by the split
+            w = torch.cat([w, w.new_zeros(64 - w.shape[0] % 64, *w.shape[1:])], 0)
+        y = _ConvFn.apply(upsample_bilinear(x, size), w, 1, 2)
         return split_channels(y, [c, c])
 
     def conv1_2_nhwc(self, x1):
@@ -546,22 +489,21 @@ def _hw(t):
 
 class D(torch.nn.Module):
     """nyud2-dir/models/modules.py:61-94: 1x1 conv + BN + ReLU on x_block4, then four up-projections to the sizes of
-    x_block3, x_block2, x_block1 and twice x_block1.  Takes resnet.E_resnet's NHWC bf16 block outputs;
-    fused_upsample as UpProjection's."""
+    x_block3, x_block2, x_block1 and twice x_block1.  Takes resnet.E_resnet's NHWC bf16 block outputs."""
 
-    def __init__(self, num_features=2048, fused_upsample=False):
+    def __init__(self, num_features=2048):
         super().__init__()
         nn = torch.nn
         self.conv = nn.Conv2d(num_features, num_features // 2, kernel_size=1, stride=1, bias=False)
         num_features = num_features // 2
         self.bn = nn.BatchNorm2d(num_features)
-        self.up1 = UpProjection(num_features, num_features // 2, fused_upsample)
+        self.up1 = UpProjection(num_features, num_features // 2)
         num_features = num_features // 2
-        self.up2 = UpProjection(num_features, num_features // 2, fused_upsample)
+        self.up2 = UpProjection(num_features, num_features // 2)
         num_features = num_features // 2
-        self.up3 = UpProjection(num_features, num_features // 2, fused_upsample)
+        self.up3 = UpProjection(num_features, num_features // 2)
         num_features = num_features // 2
-        self.up4 = UpProjection(num_features, num_features // 2, fused_upsample)
+        self.up4 = UpProjection(num_features, num_features // 2)
 
     def forward(self, x_block1, x_block2, x_block3, x_block4):
         x_d0 = _bn(conv2d_nhwc(x_block4, self.conv.weight, 1, 0), self.bn, True, self.training)
@@ -574,15 +516,15 @@ class D(torch.nn.Module):
 
 class MFF(torch.nn.Module):
     """nyud2-dir/models/modules.py:96-128: each block output up-projected to `size` with 16 channels, concatenated,
-    then 5x5 conv + BN + ReLU.  Takes resnet.E_resnet's NHWC bf16 block outputs; fused_upsample as UpProjection's."""
+    then 5x5 conv + BN + ReLU.  Takes resnet.E_resnet's NHWC bf16 block outputs."""
 
-    def __init__(self, block_channel, num_features=64, fused_upsample=False):
+    def __init__(self, block_channel, num_features=64):
         super().__init__()
         nn = torch.nn
-        self.up1 = UpProjection(block_channel[0], 16, fused_upsample)
-        self.up2 = UpProjection(block_channel[1], 16, fused_upsample)
-        self.up3 = UpProjection(block_channel[2], 16, fused_upsample)
-        self.up4 = UpProjection(block_channel[3], 16, fused_upsample)
+        self.up1 = UpProjection(block_channel[0], 16)
+        self.up2 = UpProjection(block_channel[1], 16)
+        self.up3 = UpProjection(block_channel[2], 16)
+        self.up4 = UpProjection(block_channel[3], 16)
         self.conv = nn.Conv2d(num_features, num_features, kernel_size=5, stride=1, padding=2, bias=False)
         self.bn = nn.BatchNorm2d(num_features)
 

@@ -336,24 +336,6 @@ int dirb200_conv_wgrad(const void* x, const void* dy, float* dw, void* workspace
                        int n, int h, int w, int cin, int cout, int kh, int kw, int stride, int pad,
                        int stem, int accumulate, void* stream);
 
-/* 5x5 / stride-1 / pad-2 convolutions over up = F.upsample(x, size=(ho, wo), mode='bilinear') (align_corners = False)
- * of x NHWC bf16 [n, h, w, cin]: the first half of NYUD2-DIR's _UpProjection (nyud2-dir/models/modules.py:23-27,
- * x = F.upsample(x, size); conv1(x), conv2(x)).  The up-sampled operand is formed in the conv's producer warps, with the
- * arithmetic of dirb200_upsample_bilinear_fwd (bit-identical values), and never stored; the wgrad forms it again from
- * x, so nothing at output resolution is kept for the backward.  With the tile and split-K plans of dirb200_conv_fprop /
- * _wgrad on the stored up, each result equals dirb200_upsample_bilinear_fwd followed by that call, to the bit.  The data
- * gradient d(up) is dirb200_conv_dgrad, reduced to dx by dirb200_upsample_bilinear_bwd.
- * Cin, Cout: positive multiples of 64 (conv1 and conv2 run as ONE call with their weights concatenated along Cout);
- * ho >= h, wo >= w; n <= 8192, ho, wo <= 512 and n*ho*wo < 2^31 (packed pixel of the conv kernels).  Every argument is
- * checked before any CUDA call.  y: bf16 [n, ho, wo, cout]; w_fprop from dirb200_conv_prep_weights (5x5). */
-int dirb200_conv_fprop_upsampled(const void* x, const void* w_fprop, void* y, int n, int h, int w, int cin, int cout,
-                                 int ho, int wo, void* stream);
-/* 0 for a refused shape. */
-size_t dirb200_conv_wgrad_upsampled_workspace_bytes(int n, int h, int w, int cin, int cout, int ho, int wo);
-/* dw fp32 [Cout][Cin][5][5] (=, or += when accumulate) from x and dy [n, ho, wo, cout]. */
-int dirb200_conv_wgrad_upsampled(const void* x, const void* dy, float* dw, void* workspace, size_t workspace_bytes, int n,
-                                 int h, int w, int cin, int cout, int ho, int wo, int accumulate, void* stream);
-
 /* ------------------------------------------------ Test aids: fused conv epilogues ---- */
 /* The network runner fuses BatchNorm work into the conv epilogues; these entry points run one such launch alone so
  * that it can be checked against a high-precision reference.  A statistics row layout crosses the ABI as a host

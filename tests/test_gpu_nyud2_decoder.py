@@ -1,14 +1,10 @@
 """GPU checks of NYUD2-DIR's decoder D and multi-scale fusion MFF (dense_ops.UpProjection / D / MFF,
-nyud2-dir/models/modules.py:6-31, 61-128) and of the convolution over an up-sampled operand they are built on.
+nyud2-dir/models/modules.py:6-31, 61-128).
 
-- Bit identity: dirb200_conv_fprop_upsampled / _wgrad_upsampled equal dirb200_upsample_bilinear_fwd followed by
-  dirb200_conv_fprop / _wgrad, at every up-projection shape of D and MFF at 228 x 304, plus same-size, odd and
-  non-integer scales at batch 1 and 8.
 - Fixture parity: the native modules against the reference modules' outputs and gradients (fp32 CPU fixture).
 - Teacher-forced parity at 228 x 304 (batch 2): each step of every up-projection against float64 on the same bf16
   operands, per element (conv bounds as tests/test_gpu_conv.py's).
 - Eval mode: running statistics used and left bit-unchanged (D, MFF, RefinementR).
-- With fused_upsample, no up-sampled tensor at output resolution is allocated in the forward.
 The file reruns itself with DIRB200_SMS=7 (few CTAs per conv: multi-wave tile walks, other split-K plans)."""
 import os
 import subprocess
@@ -46,74 +42,14 @@ def rel(a, b):
     return ((a.double() - b.double()).norm() / (b.double().norm() + 1e-30)).item()
 
 
-# ------------------------------------------------------------------------------------------------ bit identity
-# (n, h, w, cin, cout, ho, wo): cout is the PAIRED conv1 + conv2 width (MFF: 2 x 16 padded to 64)
-D_SHAPES = [(2, 8, 10, 1024, 1024, 15, 19), (2, 15, 19, 512, 512, 29, 38), (2, 29, 38, 256, 256, 57, 76),
-            (2, 57, 76, 128, 128, 114, 152)]
-MFF_SHAPES = [(2, 57, 76, 256, 64, 114, 152), (2, 29, 38, 512, 64, 114, 152), (2, 15, 19, 1024, 64, 114, 152),
-              (2, 8, 10, 2048, 64, 114, 152)]
-EXTRA_SHAPES = [(1, 15, 19, 64, 128, 15, 19),        # same size (scale 1)
-                (8, 15, 19, 64, 64, 15, 19),
-                (1, 7, 9, 128, 64, 20, 31),          # odd, non-integer scales
-                (8, 7, 9, 128, 1024, 20, 31),
-                (1, 5, 6, 192, 192, 13, 17),         # 3 x 64-wide column tiles
-                (8, 5, 6, 64, 128, 114, 152),
-                (8, 29, 38, 512, 64, 114, 152)]      # an MFF branch at batch 8
-BIT_SHAPES = D_SHAPES + MFF_SHAPES + EXTRA_SHAPES
-
-
-def _fused_and_composed(n, h, w, cin, cout, ho, wo, seed):
-    import _lib, _convlib  # noqa: F401
-    g = torch.Generator(device=DEV).manual_seed(seed)
-    x = torch.randn(n, h, w, cin, device=DEV, generator=g).to(torch.bfloat16)
-    wt = torch.randn(cout, cin, 5, 5, device=DEV, generator=g) * (2.0 / (25 * cin)) ** 0.5
-    dy = torch.randn(n, ho, wo, cout, device=DEV, generator=g).to(torch.bfloat16)
-    st = _lib.stream_ptr()
-    wf = torch.empty(cout, 5, 5, cin, dtype=torch.bfloat16, device=DEV)
-    _lib.call("dirb200_conv_prep_weights", _lib.ptr(wt), cout, cin, 5, 5, 0, _lib.ptr(wf), None, st)
-    up = torch.empty(n, ho, wo, cin, dtype=torch.bfloat16, device=DEV)
-    _lib.call("dirb200_upsample_bilinear_fwd", _lib.ptr(x), n, h, w, cin, ho, wo, _lib.ptr(up), st)
-    shape = (n, ho, wo, cin, cout, 5, 5, 1, 2)
-    y_ref = torch.full((n, ho, wo, cout), float("nan"), dtype=torch.bfloat16, device=DEV)
-    _lib.call("dirb200_conv_fprop", _lib.ptr(up), _lib.ptr(wf), _lib.ptr(y_ref), *shape, 0, st)
-    y = torch.full_like(y_ref, float("nan"))
-    _lib.call("dirb200_conv_fprop_upsampled", _lib.ptr(x), _lib.ptr(wf), _lib.ptr(y), n, h, w, cin, cout, ho, wo, st)
-    nb_ref = _lib.raw("dirb200_conv_wgrad_workspace_bytes")(*shape, 0)
-    nb = _lib.raw("dirb200_conv_wgrad_upsampled_workspace_bytes")(n, h, w, cin, cout, ho, wo)
-    assert nb == nb_ref > 0
-    ws = torch.empty(nb, dtype=torch.uint8, device=DEV)
-    dw_ref = torch.full((cout, cin, 5, 5), float("nan"), device=DEV)
-    _lib.call("dirb200_conv_wgrad", _lib.ptr(up), _lib.ptr(dy), _lib.ptr(dw_ref), _lib.ptr(ws), nb, *shape, 0, 0, st)
-    dw = torch.full_like(dw_ref, float("nan"))
-    _lib.call("dirb200_conv_wgrad_upsampled", _lib.ptr(x), _lib.ptr(dy), _lib.ptr(dw), _lib.ptr(ws), nb,
-              n, h, w, cin, cout, ho, wo, 0, st)
-    dw2 = dw.clone()
-    _lib.call("dirb200_conv_wgrad_upsampled", _lib.ptr(x), _lib.ptr(dy), _lib.ptr(dw2), _lib.ptr(ws), nb,
-              n, h, w, cin, cout, ho, wo, 1, st)
-    torch.cuda.synchronize()
-    return y, y_ref, dw, dw_ref, dw2
-
-
-@pytest.mark.parametrize("shape", BIT_SHAPES, ids=["x".join(map(str, s)) for s in BIT_SHAPES])
-def test_fused_conv_equals_upsample_then_conv_bitwise(shape):
-    """Fused fprop / wgrad == upsample_bilinear_fwd + conv_fprop / conv_wgrad, every bit (NaN-filled outputs: every
-    element written); accumulate mode adds the same partial sums once more."""
-    y, y_ref, dw, dw_ref, dw2 = _fused_and_composed(*shape, seed=sum(shape))
-    assert not torch.isnan(y_ref.float()).any() and not torch.isnan(dw_ref).any()
-    assert torch.equal(y.view(torch.int16), y_ref.view(torch.int16)), (y.float() - y_ref.float()).abs().max().item()
-    assert torch.equal(dw.view(torch.int32), dw_ref.view(torch.int32)), (dw - dw_ref).abs().max().item()
-    # accumulate: dw + the same reduction (the reduce adds one fp32 value per element)
-    assert torch.allclose(dw2, 2 * dw, rtol=4 * U, atol=0)
-
-
 # --------------------------------------------------------------------------------------- module construction
 CHANNELS = (256, 512, 1024, 2048)
 
 
-def make_modules(seed=0, fused=False):
+def make_modules(seed=0):
     from dense_ops import D, MFF
     torch.manual_seed(seed)
-    Dm, Mm = D(2048, fused_upsample=fused), MFF(list(CHANNELS), fused_upsample=fused)
+    Dm, Mm = D(2048), MFF(list(CHANNELS))
     with torch.no_grad():                     # non-trivial BN affine
         for mod in (Dm, Mm):
             for n, p in mod.named_parameters():
@@ -257,11 +193,10 @@ def _up_projection_teacher_forced(up, x, size, g_out):
     return out.detach()
 
 
-@pytest.mark.parametrize("fused", [False, True], ids=["stored", "fused"])
-def test_teacher_forced_layerwise_at_228x304(fused):
+def test_teacher_forced_layerwise_at_228x304():
     """Every step of every up-projection of D and MFF at 228 x 304, batch 2, on the native operands of that step,
-    against float64 (forward and backward), with the up-sampled input stored and with it formed inside the conv."""
-    Dm, Mm = make_modules(fused=fused)
+    against float64 (forward and backward)."""
+    Dm, Mm = make_modules()
     Dm.train(), Mm.train()
     xs = encoder_blocks(2, 228, 304)
     import dense_ops as O
@@ -386,38 +321,6 @@ def test_eval_bn_backward_per_element(join):
         A_b = dz.abs().reshape(-1, c).sum(0)
         _check(f"dgamma{i}", bn.weight.grad, ref_dg, (rows + 8) * U * A_g)
         _check(f"dbeta{i}", bn.bias.grad, ref_db, rows * U * A_b)
-
-
-# ------------------------------------------------------------------------------ no up-sampled tensor stored
-def test_fused_forward_allocates_no_upsampled_tensor():
-    """D + MFF forward (train mode, batch 2, 228 x 304) with fused_upsample: no allocation has the shape of an MFF
-    branch's up-sampled input (2, 114, 152, Cin), Cin = 256 ... 2048.  In D the paired conv output (2 x Cout = Cin
-    channels) has the up-sampled input's shape, so there each level allocates one tensor of that shape.  The stored
-    form (the default) is seen allocating them: two per D level, all four MFF inputs."""
-    from torch.utils._python_dispatch import TorchDispatchMode
-
-    class Shapes(TorchDispatchMode):
-        def __init__(self):
-            super().__init__()
-            self.seen = []
-
-        def __torch_dispatch__(self, func, types, args=(), kwargs=None):
-            out = func(*args, **(kwargs or {}))
-            if isinstance(out, torch.Tensor):
-                self.seen.append(tuple(out.shape))
-            return out
-
-    xs = encoder_blocks(2, 228, 304)
-    mff_up = [(2, 114, 152, c) for c in CHANNELS]
-    d_up = [(2, 15, 19, 1024), (2, 29, 38, 512), (2, 57, 76, 256), (2, 114, 152, 128)]
-    for fused, per_level, mff_count in ((True, 1, 0), (False, 2, 1)):
-        Dm, Mm = make_modules(fused=fused)
-        with Shapes() as rec:
-            d = Dm(*xs)
-        assert [rec.seen.count(s) for s in d_up] == [per_level] * 4, (fused, [rec.seen.count(s) for s in d_up])
-        with Shapes() as rec:
-            Mm(*xs, (d.shape[1], d.shape[2]))
-        assert [rec.seen.count(s) for s in mff_up] == [mff_count] * 4, (fused, [rec.seen.count(s) for s in mff_up])
 
 
 @pytest.mark.parametrize("env", [{"DIRB200_SMS": "7"}], ids=["sms7"])

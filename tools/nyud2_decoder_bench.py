@@ -4,15 +4,14 @@ forward + backward with seeded output gradients on E_resnet-shaped NHWC bf16 blo
 
   stored    the modules' default: each up-projection's input up-sampled and stored, then conv1 + conv2 as ONE
             convolution (weights concatenated along Cout)
-  fused     fused_upsample=True: the same paired convolution, with the up-sampled input formed inside the conv
-            (never stored)
   unfused   the plain composition: the stored up-sample, then conv1 and conv2 as two conv2d_nhwc calls (16-channel
             convolutions padded to 64 each)
   reference the reference's own D / MFF under torch fp32 / cuDNN with TF32 on (NCHW), where __graft_entry__.build()
             copied them into oracle/_ref (oracle/encoder_ref.py); reported as not measured otherwise
 
-The three forms alternate within one run (--rounds rounds of --steps steps each); each figure is the median step time
-over rounds, with the peak memory allocated during a step.  Prints one JSON line with the card name and power limit.
+The two native forms alternate within one run (--rounds rounds of --steps steps each); each figure is the median step
+time over rounds, with the peak memory allocated during a step.  Prints one JSON line with the card name and power
+limit.
 
     python tools/nyud2_decoder_bench.py [--steps 5] [--warmup 2] [--rounds 3]
 """
@@ -124,7 +123,7 @@ def main():
     a = ap.parse_args()
     import dense_ops as O
     paired = O.UpProjection.branch_convs
-    forms = (("stored", False, paired), ("fused", True, paired), ("unfused", False, unfused_branch_convs))
+    forms = (("stored", paired), ("unfused", unfused_branch_convs))
     out = {"tool": "nyud2_decoder_bench", **card(), "shapes": []}
     for n, h, w in SHAPES:
         torch.manual_seed(0)
@@ -133,24 +132,21 @@ def main():
         step = native_step(Dm, Mm, xs)
         res = {"n": n, "h": h, "w": w}
 
-        def use(fused, branch):
+        def use(branch):
             O.UpProjection.branch_convs = branch
-            for m in list(Dm.modules()) + list(Mm.modules()):
-                if isinstance(m, O.UpProjection):
-                    m.fused_upsample = fused
-        for form, fused, branch in forms:
-            use(fused, branch)
+        for form, branch in forms:
+            use(branch)
             res[f"{form}_ms"], res[f"{form}_peak_gib"] = [], 0.0
             for _ in range(a.warmup):
                 step()
         for _ in range(a.rounds):
-            for form, fused, branch in forms:
-                use(fused, branch)
+            for form, branch in forms:
+                use(branch)
                 ms, gb = time_steps(step, a.steps)
                 res[f"{form}_ms"].append(round(ms, 2))
                 res[f"{form}_peak_gib"] = round(max(res[f"{form}_peak_gib"], gb), 2)
-        use(False, paired)
-        for form, _, _ in forms:
+        use(paired)
+        for form, _ in forms:
             res[f"{form}_median_ms"] = statistics.median(res[f"{form}_ms"])
         del Dm, Mm, xs, step
         torch.cuda.empty_cache()

@@ -260,7 +260,7 @@ int dirb200_lds_weights_sharded(const float* labels, int64_t n, int64_t n_total,
                  "lds_weights: reweight must be sqrt_inv or inverse");
   DIRB_CHECK_ARG(n > 0 && n_total >= n && max_target > 0 && max_target <= 8192 && labels && hist && scratch && weights_out,
                  "lds_weights: bad arguments");
-  DIRB_CHECK_ARG(ks == 0 || (window_host && (ks & 1) && ks <= 33), "lds_weights: ks must be 0 or odd <= 33");
+  DIRB_CHECK_ARG(ks == 0 || (window_host && ks > 0 && (ks & 1) && ks <= 33), "lds_weights: ks must be 0 or odd <= 33");
   LdsWindow w;
   for (int i = 0; i < 33; ++i) w.w[i] = (i < ks) ? window_host[i] : 0.0;
   for (int i = 0; i < ks / 2; ++i)

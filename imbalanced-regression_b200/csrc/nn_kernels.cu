@@ -883,6 +883,83 @@ adam_kernel(float* __restrict__ p, const float* __restrict__ g, float* __restric
   }
 }
 
+// One element of the multi-tensor Adam: adam_kernel's arithmetic with the last update written as one fma.  adam_kernel
+// leaves `p -= step_size * q` to the compiler, which fuses it for some float4 lanes and not for others, so a parameter
+// may differ from the flat step's by the rounding of step_size * q (about one ulp); m and v are the same bits.
+__device__ __forceinline__ void adam_update(float& p, float gr, float& m, float& v, float beta1, float beta2, float eps,
+                                            float weight_decay, float step_size, float bc2_sqrt) {
+  if (weight_decay != 0.f) gr = fmaf(weight_decay, p, gr);
+  m = fmaf(beta1, m, (1.f - beta1) * gr);
+  v = fmaf(beta2, v, (1.f - beta2) * gr * gr);
+  const float denom = sqrtf(v) / bc2_sqrt + eps;
+  p = fmaf(-step_size, m / denom, p);
+}
+
+// Multi-tensor Adam: the segment table travels by value in the kernel's parameter block (no host-to-device copy, so a
+// step is graph-capturable).  Each segment is cut into kAdamChunk-element chunks; chunk_start[s] is the first chunk of
+// segment s and chunk_start[nseg] the total.  A CTA walks chunks grid-stride and finds each chunk's segment by binary
+// search over the prefix.  Chunks start at multiples of 4 elements, so a segment whose four pointers are 16-byte aligned
+// is read with float4s; any other segment (a view at a 4-byte offset) element by element.
+constexpr int kAdamChunk = 4096;
+constexpr int kAdamMultiMaxSegs = 512;
+
+struct AdamMultiArgs {
+  dirb200_adam_segment seg[kAdamMultiMaxSegs];
+  int chunk_start[kAdamMultiMaxSegs + 1];
+  int nseg;
+  float lr, beta1, beta2, eps, weight_decay;
+};
+// CUDA >= 12.1 allows 32764 bytes of kernel parameters on sm_70 and newer
+static_assert(sizeof(AdamMultiArgs) <= 32764, "adam_multi_kernel's parameter block is too large");
+
+__global__ void __launch_bounds__(256) adam_multi_kernel(const __grid_constant__ AdamMultiArgs a) {
+  const int total = a.chunk_start[a.nseg];
+  for (int c = blockIdx.x; c < total; c += gridDim.x) {
+    int lo = 0, hi = a.nseg - 1;                    // the last segment whose first chunk is <= c
+    while (lo < hi) {
+      const int mid = (lo + hi + 1) >> 1;
+      if (a.chunk_start[mid] <= c) lo = mid; else hi = mid - 1;
+    }
+    const dirb200_adam_segment& s = a.seg[lo];
+    float* __restrict__ p = s.param;
+    const float* __restrict__ g = s.grad;
+    float* __restrict__ m = s.exp_avg;
+    float* __restrict__ v = s.exp_avg_sq;
+    const int64_t begin = (int64_t)(c - a.chunk_start[lo]) * kAdamChunk;
+    const int64_t len = s.numel - begin < kAdamChunk ? s.numel - begin : kAdamChunk;
+    const float step_size = a.lr / s.bc1, bc2_sqrt = s.bc2_sqrt;
+    int64_t scalar_from = begin;
+    if (((reinterpret_cast<uintptr_t>(p) | reinterpret_cast<uintptr_t>(g) | reinterpret_cast<uintptr_t>(m) |
+          reinterpret_cast<uintptr_t>(v)) & 15) == 0) {
+      const int n4 = (int)(len / 4);
+      const int64_t b4 = begin / 4;
+      for (int i = threadIdx.x; i < n4; i += blockDim.x) {
+        float4 pp = reinterpret_cast<float4*>(p)[b4 + i];
+        const float4 gg = reinterpret_cast<const float4*>(g)[b4 + i];
+        float4 mm = reinterpret_cast<float4*>(m)[b4 + i], vv = reinterpret_cast<float4*>(v)[b4 + i];
+        float* pa = &pp.x;
+        const float* ga = &gg.x;
+        float* ma = &mm.x;
+        float* va = &vv.x;
+#pragma unroll
+        for (int j = 0; j < 4; ++j)
+          adam_update(pa[j], ga[j], ma[j], va[j], a.beta1, a.beta2, a.eps, a.weight_decay, step_size, bc2_sqrt);
+        reinterpret_cast<float4*>(p)[b4 + i] = pp;
+        reinterpret_cast<float4*>(m)[b4 + i] = mm;
+        reinterpret_cast<float4*>(v)[b4 + i] = vv;
+      }
+      scalar_from = begin + (int64_t)n4 * 4;
+    }
+    for (int64_t i = scalar_from + threadIdx.x; i < begin + len; i += blockDim.x) {
+      float pi = p[i], mi = m[i], vi = v[i];
+      adam_update(pi, g[i], mi, vi, a.beta1, a.beta2, a.eps, a.weight_decay, step_size, bc2_sqrt);
+      m[i] = mi;
+      v[i] = vi;
+      p[i] = pi;
+    }
+  }
+}
+
 // torch.optim.SGD with momentum (dampening 0, no nesterov), weight decay
 __global__ void __launch_bounds__(256)
 sgd_kernel(float* __restrict__ p, const float* __restrict__ g, float* __restrict__ buf, int64_t n, float lr,
@@ -1411,6 +1488,49 @@ int dirb200_adam_step(float* params, const float* grads, float* exp_avg, float* 
                                                                eps, weight_decay, (float)bc1, (float)sqrt(bc2),
                                                                grad_scale, clip_coef);
   DIRB_LAUNCHED();
+  return DIRB200_OK;
+}
+
+int dirb200_adam_step_multi(const dirb200_adam_segment* segs_host, int nseg, float lr, float beta1, float beta2,
+                            float eps, float weight_decay, void* stream) {
+  DIRB_CHECK_ARG(segs_host && nseg > 0, "adam_step_multi: bad arguments (segs_host %p, nseg %d)", (const void*)segs_host,
+                 nseg);
+  for (int k = 0; k < nseg; ++k) {
+    const dirb200_adam_segment& s = segs_host[k];
+    DIRB_CHECK_ARG(s.param && s.grad && s.exp_avg && s.exp_avg_sq, "adam_step_multi: segment %d has a null pointer", k);
+    DIRB_CHECK_ARG(((reinterpret_cast<uintptr_t>(s.param) | reinterpret_cast<uintptr_t>(s.grad) |
+                     reinterpret_cast<uintptr_t>(s.exp_avg) | reinterpret_cast<uintptr_t>(s.exp_avg_sq)) & 3) == 0,
+                   "adam_step_multi: segment %d is not 4-byte aligned", k);
+    DIRB_CHECK_ARG(s.numel > 0 && (s.numel - 1) / kAdamChunk < INT32_MAX,
+                   "adam_step_multi: segment %d has numel %lld (1 .. 2^31 chunks of %d)", k, (long long)s.numel,
+                   kAdamChunk);
+    DIRB_CHECK_ARG(isfinite(s.bc1) && s.bc1 > 0.f && isfinite(s.bc2_sqrt) && s.bc2_sqrt > 0.f,
+                   "adam_step_multi: segment %d has bias corrections bc1 %g, bc2_sqrt %g (finite and positive)", k,
+                   (double)s.bc1, (double)s.bc2_sqrt);
+  }
+  AdamMultiArgs a;
+  a.lr = lr;
+  a.beta1 = beta1;
+  a.beta2 = beta2;
+  a.eps = eps;
+  a.weight_decay = weight_decay;
+  // a launch takes up to kAdamMultiMaxSegs segments, as long as its chunk count fits the int prefix
+  for (int k = 0; k < nseg;) {
+    int ns = 0;
+    int64_t chunks = 0;
+    a.chunk_start[0] = 0;
+    while (k < nseg && ns < kAdamMultiMaxSegs) {
+      const int64_t c = (segs_host[k].numel + kAdamChunk - 1) / kAdamChunk;
+      if (ns > 0 && chunks + c > INT32_MAX) break;
+      a.seg[ns] = segs_host[k];
+      chunks += c;
+      a.chunk_start[++ns] = (int)chunks;
+      ++k;
+    }
+    a.nseg = ns;
+    adam_multi_kernel<<<grid1d(chunks, 1), 256, 0, as_stream(stream)>>>(a);
+    DIRB_LAUNCHED();
+  }
   return DIRB200_OK;
 }
 

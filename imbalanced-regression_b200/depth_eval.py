@@ -5,8 +5,13 @@ mask, copies the selected pixels to the host (one sync per image), bins every pi
 RMSE / ABS_REL / LG10 / MAE / delta1-3 on CPU tensors, overall and per many / medium / few-shot group.  Here one
 kernel (dirb200_depth_metrics_accumulate) does the up-sampling, the mask, the binning and the error sums per batch
 and adds them into a [4][10] fp64 device accumulator; evaluate_shot() copies that accumulator to the host once.
+
+Run as a script it is nyud2-dir/test.py: `python depth_eval.py --eval_model CKPT --data_dir DIR` evaluates a
+checkpoint written by nyud2_train.py (or by the reference) on the test set.
 """
+import argparse
 import logging
+import os
 
 import numpy as np
 import torch
@@ -16,6 +21,14 @@ import _lib
 SHOTS = ('overall', 'many', 'medium', 'few')
 METRICS = ('MSE', 'RMSE', 'ABS_REL', 'LG10', 'MAE', 'DELTA1', 'DELTA2', 'DELTA3', 'NUM')
 NBINS = 100                         # Evaluator.get_bin_idx clamps to 99
+# the many / medium / few-shot depth bins the reference's Evaluator hard-codes (nyud2-dir/util.py:37-44)
+SHOT_IDX = {
+    'many': [9, 10, 11, 12, 13, 14, 15, 16, 17, 18, 19, 20, 21, 22, 23, 24, 25, 26, 27, 28, 29, 30, 31, 32, 33, 34, 35,
+             36, 37, 38, 39, 40, 41, 42, 43, 44, 45, 47, 49],
+    'medium': [7, 8, 46, 48, 50, 51, 52, 53, 54, 55, 56, 58, 60, 61, 63],
+    'few': [0, 1, 2, 3, 4, 5, 6, 57, 59, 62, 64, 65, 66, 67, 68, 69, 70, 71, 72, 73, 74, 75, 76, 77, 78, 79, 80, 81, 82,
+            83, 84, 85, 86, 87, 88, 89, 90, 91, 92, 93, 94, 95, 96, 97, 98, 99],
+}
 _INT_MAX = 2 ** 31 - 1
 
 
@@ -180,3 +193,40 @@ def test(test_loader, model, shot_idx):
     logging.info('Finished testing. Start printing statistics below...')
     metric_dict = evaluator.evaluate_shot()
     return metric_dict['overall']['RMSE'], metric_dict
+
+
+def define_model():
+    """test.py:62-67: net.model without FDS around a ResNet-50 encoder (the weights come from the checkpoint)."""
+    import net
+    import resnet
+    return net.model(None, resnet.E_resnet(resnet.resnet50()), num_features=2048, block_channel=[256, 512, 1024, 2048])
+
+
+def strip_module(state_dict):
+    """A state_dict without DataParallel's `module.` prefix (keys without it pass through)."""
+    return {(k[len('module.'):] if k.startswith('module.') else k): v for k, v in state_dict.items()}
+
+
+def main(argv=None):
+    """test.py:14-37: load --eval_model into net.model (strict=False, with or without the `module.` prefix) and
+    evaluate it on --data_dir's test set.  Returns (overall RMSE, metric_dict)."""
+    parser = argparse.ArgumentParser()
+    parser.add_argument('--eval_model', type=str, default='', help='evaluation model path')
+    parser.add_argument('--data_dir', type=str, default='./data', help='data directory')
+    args = parser.parse_args(argv)
+
+    logging.root.handlers = []
+    logging.basicConfig(level=logging.INFO, format="%(asctime)s | %(message)s", handlers=[logging.StreamHandler()])
+
+    import loaddata
+    assert os.path.isfile(args.eval_model), f"No checkpoint found at '{args.eval_model}'"
+    model = define_model().cuda()
+    model_state = torch.load(args.eval_model, map_location='cpu')
+    logging.info(f"Loading checkpoint from {args.eval_model}")
+    model.load_state_dict(strip_module(model_state['state_dict']), strict=False)
+    logging.info('Loaded successfully!')
+    return test(loaddata.getTestingData(args, 1), model, SHOT_IDX)
+
+
+if __name__ == '__main__':
+    main()

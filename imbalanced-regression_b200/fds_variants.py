@@ -34,6 +34,13 @@ class FDSDepth(FDS):
         b, c, h, w = features.shape
         return features.permute(0, 2, 3, 1).contiguous().view(-1, c), labels.reshape(-1)
 
+    def accumulate_map(self, features, labels):
+        """One batch of a streamed collection (begin_epoch_stats / finish_epoch_stats): features [N, C, h, w], labels
+        the depth [N, 1, h, w], one row per pixel.  The depth rule ignores the edge flags, so begin_epoch_stats may be
+        given no labels."""
+        rows, lab = self._rows(features, labels)
+        self.accumulate_batch(rows, lab)
+
     def update_running_stats(self, features, labels, epoch):
         if epoch < self._epoch_host:
             return

@@ -499,6 +499,30 @@ int dirb200_adam_step(float* params, const float* grads, float* exp_avg, float* 
 int dirb200_sgd_step(float* params, const float* grads, float* momentum_buf, int64_t n, float lr, float momentum,
                      float weight_decay, int first_step, float grad_scale, const float* clip_coef, void* stream);
 
+/* One tensor of a multi-tensor Adam step: four fp32 device buffers of numel elements (any 4-byte alignment; 16-byte
+ * aligned ones are read with 128-bit accesses) and the tensor's own bias corrections for its step count t, computed by
+ * the caller in double precision as dirb200_adam_step does: bc1 = 1 - beta1^t, bc2_sqrt = sqrt(1 - beta2^t), each
+ * rounded to float. */
+typedef struct dirb200_adam_segment {
+  float* param;
+  const float* grad;
+  float* exp_avg;
+  float* exp_avg_sq;
+  int64_t numel;
+  float bc1;
+  float bc2_sqrt;
+} dirb200_adam_segment;
+
+/* torch.optim.Adam with coupled L2 weight decay (no amsgrad, no maximize) over a list of tensors, the replacement of
+ * torch.optim.Adam(model.parameters(), lr, weight_decay=1e-4) at nyud2-dir/train.py:146.  segs_host is a HOST array of
+ * nseg segments; it is passed by value in the kernel's parameters (one launch per 512 segments), so the call copies
+ * nothing to the device and the step is graph-capturable.  Per element the arithmetic is dirb200_adam_step's with
+ * grad_scale 1, the parameter update written as one fma: exp_avg and exp_avg_sq get the same bits as the flat step,
+ * a parameter may differ from it by about one ulp (the flat kernel's compiler fuses that update for some elements and
+ * not for others). */
+int dirb200_adam_step_multi(const dirb200_adam_segment* segs_host, int nseg, float lr, float beta1, float beta2,
+                            float eps, float weight_decay, void* stream);
+
 /* torch.nn.utils.clip_grad_norm_ over one flat gradient buffer (sts-b-dir/trainer.py:147-149, --max_grad_norm):
  * out[0] = min(1, max_norm / (||grad_scale * grads||_2 + 1e-6)), out[1] = that norm.  The gradients themselves are
  * not rewritten -- the optimizer step applies out[0] while it reads them.  workspace: >= 8 KiB + 16 B, fp64 partials. */

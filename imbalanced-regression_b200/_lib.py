@@ -86,6 +86,18 @@ _SIGS = {
     "dirb200_depth_augment_workspace_bytes": (c_size_t, [c_int, c_int, c_int, c_int, c_int]),
     "dirb200_depth_augment_batch": (c_int, [P, P, c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_int, P, P, P, P,
                                             P, P, P, c_int, P, P, P, P, P, P, c_size_t, P]),
+    # STS-B-DIR sentence-pair encoder (csrc/lstm.cu, csrc/pair_encoder.cu)
+    "dirb200_lstm_prep_weights": (c_int, [P] * 8 + [c_int] * 5 + [P] * 6),
+    "dirb200_lstm_scatter_grads": (c_int, [P] * 3 + [c_int] * 5 + [P] * 9),
+    "dirb200_lstm_fwd_step": (c_int, [P, P, P, P] + [c_int] * 5 + [P] * 5),
+    "dirb200_lstm_layer_fwd": (c_int, [P, P, P, P] + [c_int] * 4 + [P] * 5),
+    "dirb200_lstm_bwd_step": (c_int, [P] * 5 + [c_int] * 4 + [P] * 4),
+    "dirb200_lstm_layer_bwd": (c_int, [P] * 5 + [c_int] * 3 + [P] * 4),
+    "dirb200_col_sum_bf16": (c_int, [P, c_int64, c_int, P, P]),
+    "dirb200_embed_gather": (c_int, [P, P, P, P, c_int64, c_int, c_int, c_int, c_int, P, P]),
+    "dirb200_embed_grad": (c_int, [P, P, P, P, c_int64, c_int, c_int, c_int, c_int, c_int64, P, P]),
+    "dirb200_pair_maxpool_fwd": (c_int, [P, P, P, c_int, c_int, c_int, c_int, P, P, P]),
+    "dirb200_pair_maxpool_bwd": (c_int, [P, P, P, P, c_int, c_int, c_int, c_int, P, P]),
 }
 
 

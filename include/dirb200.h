@@ -530,6 +530,61 @@ size_t dirb200_grad_clip_workspace_bytes(void);
 int dirb200_grad_clip_coef(const float* grads, int64_t n, float grad_scale, float max_norm, void* workspace,
                            size_t workspace_bytes, float* out, void* stream);
 
+/* ------------------------------------------- STS-B-DIR sentence-pair encoder ---- */
+/* The 2-layer bidirectional LSTM of sts-b-dir/models.py:40-43 (nn.LSTM(d_word, d_hid, n_layers_enc,
+ * bidirectional=True) run packed by the masked seq2seq wrapper) and the masked max-pool + pair features of
+ * models.py:155-166.  Layouts and the gate interleaving are described in csrc/lstm.cu; rows M = 2B (s1 then s2),
+ * lengths int32 in [1, T] (the caller checks), Hp / Dp the hidden / input sizes padded to multiples of 64.
+ * T <= 4096, M <= 65535, Hp <= 4096. */
+/* One layer's fp32 weights, both directions (torch layout, gate order i, f, g, o), -> bf16 GEMM operands:
+ * w_ih [2*4Hp][Dp] (conv_fprop operand), w_ih_t [Dp][2*4Hp] (conv_dgrad operand), w_hh [2][4Hp][Hp],
+ * w_hh_t [2][Hp][4Hp], bias fp32 [2][4Hp] = b_ih + b_hh.  The input has in_blocks blocks of din / in_blocks real
+ * columns, each padded to Dp / in_blocks (layer 0: 1 block of d_word; later layers: the 2 directions' outputs).
+ * Padding is zero. */
+int dirb200_lstm_prep_weights(const float* w_ih_f, const float* w_hh_f, const float* b_ih_f, const float* b_hh_f,
+                              const float* w_ih_r, const float* w_hh_r, const float* b_ih_r, const float* b_hh_r,
+                              int H, int din, int in_blocks, int Hp, int Dp, void* w_ih, void* w_ih_t, void* w_hh,
+                              void* w_hh_t, float* bias, void* stream);
+/* Inverse of the re-layout for fp32 gradients: dw_ih [2*4Hp][Dp], dw_hh [2][4Hp][Hp], db [2][4Hp] -> the eight
+ * torch-layout gradients (overwritten; db goes to both bias_ih and bias_hh). */
+int dirb200_lstm_scatter_grads(const float* dw_ih, const float* dw_hh, const float* db, int H, int din, int in_blocks,
+                               int Hp, int Dp, float* gw_ih_f, float* gw_hh_f, float* gb_ih_f, float* gb_hh_f,
+                               float* gw_ih_r, float* gw_hh_r, float* gb_ih_r, float* gb_hh_r, void* stream);
+/* Recurrent forward step s of both directions (one launch): gates = h_s . W_hh^T + xproj + bias, the cell update,
+ * h_{s+1}, c_{s+1} and the output y at the step's time.  save != 0: h / c have T + 1 slots and the activated gates
+ * (fp32) are kept for the backward; save == 0: 2 slots, gates unused.  dirb200_lstm_layer_fwd zeroes slot 0 and runs
+ * every step, one launch each. */
+int dirb200_lstm_fwd_step(const void* xproj, const void* w_hh, const float* bias, const int* lens, int T, int M,
+                          int Hp, int save, int s, void* h, float* c, float* gates, void* y, void* stream);
+int dirb200_lstm_layer_fwd(const void* xproj, const void* w_hh, const float* bias, const int* lens, int T, int M,
+                           int Hp, int save, void* h, float* c, float* gates, void* y, void* stream);
+/* Recurrent backward step s (one launch): dh = dgates_{s+1} . W_hh + dy at the step's time, the cell backward, the
+ * pre-activation gradients dgates_s (bf16, step order dg [2][T][M][4Hp] and time order dg_time [T][M][2][4Hp]) and
+ * the carried dc (fp32, dc [2][2][M][Hp]).  dirb200_lstm_layer_bwd runs s = T-1 .. 0. */
+int dirb200_lstm_bwd_step(const void* w_hh_t, const void* dy, const float* gates, const float* c, const int* lens,
+                          int T, int M, int Hp, int s, float* dc, void* dg, void* dg_time, void* stream);
+int dirb200_lstm_layer_bwd(const void* w_hh_t, const void* dy, const float* gates, const float* c, const int* lens,
+                           int T, int M, int Hp, float* dc, void* dg, void* dg_time, void* stream);
+/* out[col] = sum over rows of bf16 x[rows][cols], fp32, in a fixed order (the LSTM bias gradient). */
+int dirb200_col_sum_bf16(const void* x, int64_t rows, int cols, float* out, void* stream);
+/* Embedding lookup (models.py:138, 141-142): x bf16 [T][M][Dp] = emb[ids[m][t]] * dmul[m][t] for t < lens[m], zero
+ * elsewhere; ids int64 [M][T]; dmul fp32 [M][T][D] dropout multipliers or NULL. */
+int dirb200_embed_gather(const int64_t* ids, const int* lens, const float* emb, const float* dmul, int64_t V, int M,
+                         int T, int D, int Dp, void* x, void* stream);
+/* Its gradient dw fp32 [V][D] (overwritten), deterministic: each row summed in position order m T + t.  Row
+ * padding_index (-1: none) gets no gradient, as F.embedding's padding_idx; positions with an id outside [0, V)
+ * contribute nothing. */
+int dirb200_embed_grad(const int64_t* ids, const int* lens, const void* dx, const float* dmul, int64_t V, int M, int T,
+                       int D, int Dp, int64_t padding_index, float* dw, void* stream);
+/* Masked max over time and pair features (models.py:155-166): y bf16 [T][2B][2Hp] (layer output), dmul fp32
+ * [2B][T][2H] or NULL -> feat fp32 [B][8H] = [u, v, |u - v|, u * v], arg int32 [2B][2H] the argmax time (first
+ * maximal t on ties). */
+int dirb200_pair_maxpool_fwd(const void* y, const int* lens, const float* dmul, int B, int T, int H, int Hp,
+                             float* feat, int* arg, void* stream);
+/* Its backward: dy bf16 [T][2B][2Hp] (zeroed here) gets the gradient at each argmax. */
+int dirb200_pair_maxpool_bwd(const float* gfeat, const float* feat, const int* arg, const float* dmul, int B, int T,
+                             int H, int Hp, void* dy, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

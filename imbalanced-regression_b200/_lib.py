@@ -57,6 +57,8 @@ _SIGS = {
     "dirb200_lds_weights_sharded": (c_int, [P, c_int64, c_int64, c_int, c_int, P, c_int, P, P, P, P]),
     "dirb200_int_label_histogram": (c_int, [P, c_int64, c_int, P, P]),
     "dirb200_shot_metrics": (c_int, [P, P, c_int64, P, c_int, c_int, c_int, P, P]),
+    "dirb200_stsb_shot_metrics_workspace_bytes": (c_size_t, [c_int64]),
+    "dirb200_stsb_shot_metrics": (c_int, [P, P, c_int64, P, c_size_t, P, P]),
     "dirb200_depth_metrics_workspace_bytes": (c_size_t, [c_int64, c_int, c_int]),
     "dirb200_depth_metrics_accumulate": (c_int, [P, c_int, c_int, P, P, c_int64, c_int, c_int, P, c_int, P, P,
                                                  c_size_t, P]),

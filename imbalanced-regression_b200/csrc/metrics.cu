@@ -12,6 +12,7 @@
 // 0) and to "median" otherwise.  Here: one exact int64 histogram of int(train_label), then one pass over the test
 // samples accumulating, per group, (count, sum d^2, sum |d|, sum log|d|) in fp64.
 #include "common.cuh"
+#include "bins.cuh"
 
 namespace dirb200 {
 
@@ -225,6 +226,192 @@ depth_metrics_kernel(DepthEvalArgs a, double* __restrict__ acc_out, double* __re
   }
 }
 
+// ------------------------------------------------------------------------------------------------------------------
+// STS-B-DIR's STSShotAverage.get_metric (sts-b-dir/util.py:101-172): count, MSE, L1, G-mean, Pearson and Spearman over
+// x = 5 pred (fp64) and y = label, overall and per many / medium / few group.  A label's group is its bin under the
+// DIRB200_BIN_EDGES5 rule with 50 bins (util.py:115-120: np.histogram edges over [0, 5], 5.0 in the last bin) looked
+// up in util.py:110-113's table.  A negative label, whose reference bin is -1, is in no list and so counts as few.
+//
+// Spearman is Pearson of the average ranks within each group (scipy's rankdata('average')).  stsb_rank_kernel gets
+// them as exact counts, 2 rank = #less + #less-or-equal + 1, from a tiled O(N^2) comparison of every pair: no sort, no
+// floating point.  The order of fp32 preds is the order of 5 pred in fp64 (exact), so the raw fp32 values are
+// compared.  stsb_metrics_kernel is one CTA: a first pass of sums, then centred sums about the means of the first, and
+// the final formulas; every sum has a fixed order, so two identical calls give identical bits.
+constexpr int kStsbGroups = 4;   // 0 overall, 1 many, 2 medium, 3 few (the order of util.py:143)
+constexpr int kStsbOut = 6;      // num_samples, mse, l1, gmean, pearsonr, spearmanr
+constexpr int64_t kStsbMaxN = 1ll << 22;
+
+__constant__ unsigned char kStsbShotOfBin[50] = {
+    // util.py:110-113, bins 0 .. 49
+    1, 3, 2, 3, 2, 3, 2, 3, 2, 3, 1, 3, 1, 3, 1, 3, 1, 3, 1, 3, 1, 3, 1, 3, 1,
+    3, 1, 2, 1, 3, 1, 3, 1, 3, 1, 2, 1, 2, 1, 3, 1, 3, 1, 3, 1, 3, 1, 3, 1, 1};
+
+__device__ __forceinline__ int stsb_group(float label) {
+  if (!(label >= 0.f)) return 3;     // bin -1 (a NaN label is out of the reference's contract: few as well)
+  return kStsbShotOfBin[bin_of(DIRB200_BIN_EDGES5, label, 0.f, 49.f, 50, false, false)];
+}
+
+// r2[i] = twice the average rank of pred_i and label_i, overall (.x, .y) and within i's group (.z, .w)
+__global__ void __launch_bounds__(256)
+stsb_rank_kernel(const float* __restrict__ preds, const float* __restrict__ labels, int n, int4* __restrict__ r2) {
+  __shared__ float sp[256], sl[256];
+  __shared__ int sg[256];
+  const int i = blockIdx.x * 256 + threadIdx.x;
+  const bool in = i < n;
+  const float p = in ? preds[i] : 0.f, l = in ? labels[i] : 0.f;
+  const int g = in ? stsb_group(l) : 0;
+  int ap = 0, al = 0, gp = 0, gl = 0;    // #less + #less-or-equal, overall and in the group
+  for (int j0 = 0; j0 < n; j0 += 256) {
+    __syncthreads();
+    const int j = j0 + threadIdx.x;
+    if (j < n) {
+      sp[threadIdx.x] = preds[j];
+      sl[threadIdx.x] = labels[j];
+      sg[threadIdx.x] = stsb_group(labels[j]);
+    }
+    __syncthreads();
+    const int m = n - j0 < 256 ? n - j0 : 256;
+#pragma unroll 4
+    for (int k = 0; k < m; ++k) {
+      const float q = sp[k], r = sl[k];
+      const int cp = (q < p) + (q <= p), cl = (r < l) + (r <= l);
+      ap += cp;
+      al += cl;
+      if (sg[k] == g) {
+        gp += cp;
+        gl += cl;
+      }
+    }
+  }
+  if (in) r2[i] = make_int4(ap + 1, al + 1, gp + 1, gl + 1);
+}
+
+// per-thread sums: [group][quantity]; a sample adds to group 0 and to its own group
+template <int K>
+__device__ __forceinline__ void stsb_add(double (&acc)[kStsbGroups][K], int g, const double (&v0)[K],
+                                         const double (&vg)[K]) {
+#pragma unroll
+  for (int k = 0; k < K; ++k) acc[0][k] += v0[k];
+#pragma unroll
+  for (int gg = 1; gg < kStsbGroups; ++gg)
+    if (gg == g) {
+#pragma unroll
+      for (int k = 0; k < K; ++k) acc[gg][k] += vg[k];
+    }
+}
+
+// sums acc over the CTA (warp shuffles, then the warps in order) into tot, visible to every thread on return
+template <int K>
+__device__ void stsb_cta_sum(double (&acc)[kStsbGroups][K], double* sh, double* tot) {
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31, nw = blockDim.x >> 5;
+#pragma unroll
+  for (int g = 0; g < kStsbGroups; ++g)
+#pragma unroll
+    for (int k = 0; k < K; ++k) {
+      const double s = warp_sum(acc[g][k]);
+      if (lane == 0) sh[warp * kStsbGroups * K + g * K + k] = s;
+    }
+  __syncthreads();
+  if (threadIdx.x < kStsbGroups * K) {
+    double t = 0.0;
+    for (int w = 0; w < nw; ++w) t += sh[w * kStsbGroups * K + threadIdx.x];
+    tot[threadIdx.x] = t;
+  }
+  __syncthreads();
+}
+
+__device__ __forceinline__ double stsb_clip_corr(double r) { return r > 1.0 ? 1.0 : (r < -1.0 ? -1.0 : r); }
+
+// rank of a sample from r2 (NaN for a NaN value: scipy's rankdata propagates it)
+__device__ __forceinline__ double stsb_rank(int twice, float v) { return v == v ? 0.5 * (double)twice : (double)NAN; }
+
+constexpr int kStsbSum1 = 8;   // n, sum x, sum y, sum rx, sum ry, sum d^2, sum |d|, sum log |d|'
+constexpr int kStsbSum2 = 8;   // Sxx, Syy, Sxy, Srxrx, Sryry, Srxry, #(x not at the constant rank), same for y
+
+__global__ void __launch_bounds__(256)
+stsb_metrics_kernel(const float* __restrict__ preds, const float* __restrict__ labels, int n,
+                    const int4* __restrict__ r2, double* __restrict__ out) {
+  __shared__ double sh[8 * kStsbGroups * kStsbSum1];
+  __shared__ double s1[kStsbGroups * kStsbSum1], s2[kStsbGroups * kStsbSum2];
+  double acc[kStsbGroups][kStsbSum1];
+#pragma unroll
+  for (int g = 0; g < kStsbGroups; ++g)
+#pragma unroll
+    for (int k = 0; k < kStsbSum1; ++k) acc[g][k] = 0.0;
+  for (int i = threadIdx.x; i < n; i += blockDim.x) {
+    const float p = preds[i], l = labels[i];
+    const int4 r = r2[i];
+    const double x = (double)p * 5.0, y = (double)l;
+    const double d = x - y, a = fabs(d);
+    const double lg = log(a == 0.0 ? 1e-10 : a);      // util.py:152-154: an exact zero difference counts as 1e-10
+    const double v0[kStsbSum1] = {1.0, x, y, stsb_rank(r.x, p), stsb_rank(r.y, l), d * d, a, lg};
+    const double vg[kStsbSum1] = {1.0, x, y, stsb_rank(r.z, p), stsb_rank(r.w, l), d * d, a, lg};
+    stsb_add(acc, stsb_group(l), v0, vg);
+  }
+  stsb_cta_sum(acc, sh, s1);
+
+  double acc2[kStsbGroups][kStsbSum2];
+#pragma unroll
+  for (int g = 0; g < kStsbGroups; ++g)
+#pragma unroll
+    for (int k = 0; k < kStsbSum2; ++k) acc2[g][k] = 0.0;
+  for (int i = threadIdx.x; i < n; i += blockDim.x) {
+    const float p = preds[i], l = labels[i];
+    const int4 r = r2[i];
+    const int g = stsb_group(l);
+    const double x = (double)p * 5.0, y = (double)l;
+    double v[2][kStsbSum2];
+#pragma unroll
+    for (int s = 0; s < 2; ++s) {
+      const int gg = s == 0 ? 0 : g;
+      const double* m = s1 + gg * kStsbSum1;
+      const double cnt = m[0];
+      const double xm = x - m[1] / cnt, ym = y - m[2] / cnt;
+      const double rx = stsb_rank(s == 0 ? r.x : r.z, p) - m[3] / cnt;
+      const double ry = stsb_rank(s == 0 ? r.y : r.w, l) - m[4] / cnt;
+      // a group's x is constant exactly when every member's twice-rank is cnt + 1 (all tied)
+      const int tx = s == 0 ? r.x : r.z, ty = s == 0 ? r.y : r.w;
+      v[s][0] = xm * xm;
+      v[s][1] = ym * ym;
+      v[s][2] = xm * ym;
+      v[s][3] = rx * rx;
+      v[s][4] = ry * ry;
+      v[s][5] = rx * ry;
+      v[s][6] = (double)tx != cnt + 1.0 ? 1.0 : 0.0;
+      v[s][7] = (double)ty != cnt + 1.0 ? 1.0 : 0.0;
+    }
+    stsb_add(acc2, g, v[0], v[1]);
+  }
+  stsb_cta_sum(acc2, sh, s2);
+
+  if (threadIdx.x < kStsbGroups) {
+    const int g = threadIdx.x;
+    const double* a = s1 + g * kStsbSum1;
+    const double* b = s2 + g * kStsbSum2;
+    const double cnt = a[0];
+    double* o = out + g * kStsbOut;
+    o[0] = cnt;
+    if (cnt == 0.0) {                      // util.py: an empty group reports 0 for every metric
+      o[1] = o[2] = o[3] = o[4] = o[5] = 0.0;
+      return;
+    }
+    o[1] = a[5] / cnt;
+    o[2] = a[6] / cnt;
+    o[3] = exp(a[7] / cnt);                // scipy.stats.gmean: exp(mean(log))
+    if (cnt < 2.0) {                       // util.py:161, 163: size 1 reports 0
+      o[4] = o[5] = 0.0;
+      return;
+    }
+    // scipy.stats.pearsonr: NaN for a constant input, the centred formula clipped to [-1, 1], rounded for n == 2
+    double pr = stsb_clip_corr(b[2] / (sqrt(b[0]) * sqrt(b[1])));
+    if (cnt == 2.0) pr = rint(pr);
+    if (b[6] == 0.0 || b[7] == 0.0) pr = (double)NAN;
+    o[4] = pr;
+    // scipy.stats.spearmanr: np.corrcoef of the ranks (all-tied ranks give 0 / 0 = NaN)
+    o[5] = stsb_clip_corr(b[5] / (sqrt(b[3]) * sqrt(b[4])));
+  }
+}
+
 }  // namespace dirb200
 
 using namespace dirb200;
@@ -254,6 +441,29 @@ int dirb200_shot_metrics(const float* preds, const float* labels, int64_t n, con
   if (g > 2 * num_sms()) g = 2 * num_sms();
   shot_metrics_kernel<<<(unsigned)g, 256, 0, st>>>(preds, labels, n, reinterpret_cast<const unsigned long long*>(train_hist),
                                                  nbins, many_shot_thr, low_shot_thr, out16);
+  DIRB_LAUNCHED();
+  return DIRB200_OK;
+}
+
+size_t dirb200_stsb_shot_metrics_workspace_bytes(int64_t n) { return n > 0 ? sizeof(int4) * (size_t)n : 0; }
+
+int dirb200_stsb_shot_metrics(const float* preds, const float* labels, int64_t n, void* workspace,
+                              size_t workspace_bytes, double* out24, void* stream) {
+  // the rank counts reach 2 n + 1 in int32, and the pair comparison is quadratic: 2^22 keeps both bounded
+  DIRB_CHECK_ARG(n >= 0 && n <= kStsbMaxN, "stsb_shot_metrics: n %lld out of range (0 .. 2^22)", (long long)n);
+  DIRB_CHECK_ARG(out24 && (n == 0 || (preds && labels && workspace)), "stsb_shot_metrics: null pointer");
+  DIRB_CHECK_ARG(reinterpret_cast<uintptr_t>(workspace) % 16 == 0, "stsb_shot_metrics: workspace must be 16-byte aligned");
+  if (workspace_bytes < dirb200_stsb_shot_metrics_workspace_bytes(n)) {
+    set_error("stsb_shot_metrics: workspace too small");
+    return DIRB200_ERR_WORKSPACE;
+  }
+  cudaStream_t st = as_stream(stream);
+  int4* r2 = reinterpret_cast<int4*>(workspace);
+  if (n > 0) {
+    stsb_rank_kernel<<<(unsigned)((n + 255) / 256), 256, 0, st>>>(preds, labels, (int)n, r2);
+    DIRB_LAUNCHED();
+  }
+  stsb_metrics_kernel<<<1, 256, 0, st>>>(preds, labels, (int)n, r2, out24);
   DIRB_LAUNCHED();
   return DIRB200_OK;
 }

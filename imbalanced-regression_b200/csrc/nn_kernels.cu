@@ -912,7 +912,12 @@ struct AdamMultiArgs {
 // CUDA >= 12.1 allows 32764 bytes of kernel parameters on sm_70 and newer
 static_assert(sizeof(AdamMultiArgs) <= 32764, "adam_multi_kernel's parameter block is too large");
 
-__global__ void __launch_bounds__(256) adam_multi_kernel(const __grid_constant__ AdamMultiArgs a) {
+// kClip: every gradient is multiplied by the device scalar *clip_coef as it is read (clipping without rewriting
+// .grad); without it the arithmetic is untouched, and a coefficient of exactly 1 gives the same bits.
+template <bool kClip>
+__global__ void __launch_bounds__(256) adam_multi_kernel(const __grid_constant__ AdamMultiArgs a,
+                                                         const float* __restrict__ clip_coef) {
+  const float coef = kClip ? *clip_coef : 1.f;
   const int total = a.chunk_start[a.nseg];
   for (int c = blockIdx.x; c < total; c += gridDim.x) {
     int lo = 0, hi = a.nseg - 1;                    // the last segment whose first chunk is <= c
@@ -943,7 +948,8 @@ __global__ void __launch_bounds__(256) adam_multi_kernel(const __grid_constant__
         float* va = &vv.x;
 #pragma unroll
         for (int j = 0; j < 4; ++j)
-          adam_update(pa[j], ga[j], ma[j], va[j], a.beta1, a.beta2, a.eps, a.weight_decay, step_size, bc2_sqrt);
+          adam_update(pa[j], kClip ? ga[j] * coef : ga[j], ma[j], va[j], a.beta1, a.beta2, a.eps, a.weight_decay,
+                      step_size, bc2_sqrt);
         reinterpret_cast<float4*>(p)[b4 + i] = pp;
         reinterpret_cast<float4*>(m)[b4 + i] = mm;
         reinterpret_cast<float4*>(v)[b4 + i] = vv;
@@ -952,7 +958,8 @@ __global__ void __launch_bounds__(256) adam_multi_kernel(const __grid_constant__
     }
     for (int64_t i = scalar_from + threadIdx.x; i < begin + len; i += blockDim.x) {
       float pi = p[i], mi = m[i], vi = v[i];
-      adam_update(pi, g[i], mi, vi, a.beta1, a.beta2, a.eps, a.weight_decay, step_size, bc2_sqrt);
+      adam_update(pi, kClip ? g[i] * coef : g[i], mi, vi, a.beta1, a.beta2, a.eps, a.weight_decay, step_size,
+                  bc2_sqrt);
       m[i] = mi;
       v[i] = vi;
       p[i] = pi;
@@ -1019,6 +1026,86 @@ grad_clip_kernel(const float* __restrict__ g, int64_t n, float scale, float max_
     out[0] = coef < 1.f ? coef : 1.f;
     out[1] = norm;
     *ticket = 0u;                          // ready for the next step
+  }
+}
+
+// Multi-tensor gradient norm: the (grad, numel) table travels by value, cut into kAdamChunk-element chunks as in
+// adam_multi_kernel.  Each thread squares a chunk's elements in fp32 (at most kAdamChunk / 256 = 16 fmas) and adds
+// that to an fp64 sum; CTA b adds its fp64 total into partials[b] (or writes it, in a call's first launch).  Every
+// launch of one call uses the same grid, and launches on one stream run in order, so no atomics are needed for that.
+// In the call's last launch the last CTA (ticket) sums partials[0 .. grid) in CTA order and writes {coef, norm}:
+// two identical calls give identical bits.
+struct GradNormArgs {
+  const float* grad[kAdamMultiMaxSegs];
+  int64_t numel[kAdamMultiMaxSegs];
+  int chunk_start[kAdamMultiMaxSegs + 1];
+  int nseg;
+  int first, last;          // this launch is the call's first / last
+  float max_norm;
+};
+static_assert(sizeof(GradNormArgs) <= 32764, "grad_norm_multi_kernel's parameter block is too large");
+
+__global__ void __launch_bounds__(256) grad_norm_multi_kernel(const __grid_constant__ GradNormArgs a,
+                                                              double* __restrict__ partials,
+                                                              unsigned int* __restrict__ ticket,
+                                                              float* __restrict__ out) {
+  __shared__ double sh[8];
+  __shared__ bool last;
+  double acc = 0.0;
+  const int total = a.chunk_start[a.nseg];
+  for (int c = blockIdx.x; c < total; c += gridDim.x) {
+    int lo = 0, hi = a.nseg - 1;                    // the last segment whose first chunk is <= c
+    while (lo < hi) {
+      const int mid = (lo + hi + 1) >> 1;
+      if (a.chunk_start[mid] <= c) lo = mid; else hi = mid - 1;
+    }
+    const float* __restrict__ g = a.grad[lo];
+    const int64_t begin = (int64_t)(c - a.chunk_start[lo]) * kAdamChunk;
+    const int64_t len = a.numel[lo] - begin < kAdamChunk ? a.numel[lo] - begin : kAdamChunk;
+    float s = 0.f;
+    int64_t scalar_from = begin;
+    if ((reinterpret_cast<uintptr_t>(g) & 15) == 0) {
+      const int n4 = (int)(len / 4);
+      const int64_t b4 = begin / 4;
+      for (int i = threadIdx.x; i < n4; i += blockDim.x) {
+        const float4 v = reinterpret_cast<const float4*>(g)[b4 + i];
+        s = fmaf(v.x, v.x, fmaf(v.y, v.y, fmaf(v.z, v.z, fmaf(v.w, v.w, s))));
+      }
+      scalar_from = begin + (int64_t)n4 * 4;
+    }
+    for (int64_t i = scalar_from + threadIdx.x; i < begin + len; i += blockDim.x) s = fmaf(g[i], g[i], s);
+    acc += (double)s;
+  }
+  double t = warp_sum(acc);
+  if ((threadIdx.x & 31) == 0) sh[threadIdx.x >> 5] = t;
+  __syncthreads();
+  if (threadIdx.x == 0) {
+    double s = 0.0;
+    for (int w = 0; w < 8; ++w) s += sh[w];
+    partials[blockIdx.x] = a.first ? s : partials[blockIdx.x] + s;
+    if (a.last) {
+      __threadfence();
+      last = atomicAdd(ticket, 1u) == gridDim.x - 1;
+    } else {
+      last = false;
+    }
+  }
+  __syncthreads();
+  if (!last) return;
+  __threadfence();
+  double tot = 0.0;
+  for (int i = threadIdx.x; i < (int)gridDim.x; i += blockDim.x) tot += ((volatile double*)partials)[i];
+  tot = warp_sum(tot);
+  if ((threadIdx.x & 31) == 0) sh[threadIdx.x >> 5] = tot;
+  __syncthreads();
+  if (threadIdx.x == 0) {
+    double s = 0.0;
+    for (int w = 0; w < 8; ++w) s += sh[w];
+    const float norm = (float)sqrt(s);
+    const float coef = a.max_norm / (norm + 1e-6f);
+    out[0] = coef < 1.f ? coef : (coef == coef ? 1.f : coef);   // torch.clamp(coef, max=1) keeps a NaN
+    out[1] = norm;
+    *ticket = 0u;                          // ready for the next call
   }
 }
 
@@ -1491,21 +1578,22 @@ int dirb200_adam_step(float* params, const float* grads, float* exp_avg, float* 
   return DIRB200_OK;
 }
 
-int dirb200_adam_step_multi(const dirb200_adam_segment* segs_host, int nseg, float lr, float beta1, float beta2,
-                            float eps, float weight_decay, void* stream) {
-  DIRB_CHECK_ARG(segs_host && nseg > 0, "adam_step_multi: bad arguments (segs_host %p, nseg %d)", (const void*)segs_host,
+// dirb200_adam_step_multi and its clipped form: the checks, then one launch per kAdamMultiMaxSegs segments
+static int adam_multi(const char* name, const dirb200_adam_segment* segs_host, int nseg, float lr, float beta1,
+                      float beta2, float eps, float weight_decay, const float* clip_coef, void* stream) {
+  DIRB_CHECK_ARG(segs_host && nseg > 0, "%s: bad arguments (segs_host %p, nseg %d)", name, (const void*)segs_host,
                  nseg);
   for (int k = 0; k < nseg; ++k) {
     const dirb200_adam_segment& s = segs_host[k];
-    DIRB_CHECK_ARG(s.param && s.grad && s.exp_avg && s.exp_avg_sq, "adam_step_multi: segment %d has a null pointer", k);
+    DIRB_CHECK_ARG(s.param && s.grad && s.exp_avg && s.exp_avg_sq, "%s: segment %d has a null pointer", name, k);
     DIRB_CHECK_ARG(((reinterpret_cast<uintptr_t>(s.param) | reinterpret_cast<uintptr_t>(s.grad) |
                      reinterpret_cast<uintptr_t>(s.exp_avg) | reinterpret_cast<uintptr_t>(s.exp_avg_sq)) & 3) == 0,
-                   "adam_step_multi: segment %d is not 4-byte aligned", k);
+                   "%s: segment %d is not 4-byte aligned", name, k);
     DIRB_CHECK_ARG(s.numel > 0 && (s.numel - 1) / kAdamChunk < INT32_MAX,
-                   "adam_step_multi: segment %d has numel %lld (1 .. 2^31 chunks of %d)", k, (long long)s.numel,
+                   "%s: segment %d has numel %lld (1 .. 2^31 chunks of %d)", name, k, (long long)s.numel,
                    kAdamChunk);
     DIRB_CHECK_ARG(isfinite(s.bc1) && s.bc1 > 0.f && isfinite(s.bc2_sqrt) && s.bc2_sqrt > 0.f,
-                   "adam_step_multi: segment %d has bias corrections bc1 %g, bc2_sqrt %g (finite and positive)", k,
+                   "%s: segment %d has bias corrections bc1 %g, bc2_sqrt %g (finite and positive)", name, k,
                    (double)s.bc1, (double)s.bc2_sqrt);
   }
   AdamMultiArgs a;
@@ -1528,10 +1616,26 @@ int dirb200_adam_step_multi(const dirb200_adam_segment* segs_host, int nseg, flo
       ++k;
     }
     a.nseg = ns;
-    adam_multi_kernel<<<grid1d(chunks, 1), 256, 0, as_stream(stream)>>>(a);
+    if (clip_coef)
+      adam_multi_kernel<true><<<grid1d(chunks, 1), 256, 0, as_stream(stream)>>>(a, clip_coef);
+    else
+      adam_multi_kernel<false><<<grid1d(chunks, 1), 256, 0, as_stream(stream)>>>(a, nullptr);
     DIRB_LAUNCHED();
   }
   return DIRB200_OK;
+}
+
+int dirb200_adam_step_multi(const dirb200_adam_segment* segs_host, int nseg, float lr, float beta1, float beta2,
+                            float eps, float weight_decay, void* stream) {
+  return adam_multi("adam_step_multi", segs_host, nseg, lr, beta1, beta2, eps, weight_decay, nullptr, stream);
+}
+
+int dirb200_adam_step_multi_clipped(const dirb200_adam_segment* segs_host, int nseg, float lr, float beta1,
+                                    float beta2, float eps, float weight_decay, const float* clip_coef,
+                                    void* stream) {
+  DIRB_CHECK_ARG(clip_coef, "adam_step_multi_clipped: clip_coef is null");
+  return adam_multi("adam_step_multi_clipped", segs_host, nseg, lr, beta1, beta2, eps, weight_decay, clip_coef,
+                    stream);
 }
 
 int dirb200_sgd_step(float* params, const float* grads, float* momentum_buf, int64_t n, float lr, float momentum,
@@ -1560,6 +1664,63 @@ int dirb200_grad_clip_coef(const float* grads, int64_t n, float grad_scale, floa
   if (grid > kClipMaxGrid) grid = kClipMaxGrid;
   grad_clip_kernel<<<grid, 256, 0, as_stream(stream)>>>(grads, n, grad_scale, max_norm, partials, ticket, out);
   DIRB_LAUNCHED();
+  return DIRB200_OK;
+}
+
+size_t dirb200_grad_norm_multi_workspace_bytes(void) { return sizeof(double) * kClipMaxGrid + 16; }
+
+int dirb200_grad_norm_multi(const dirb200_grad_segment* segs_host, int nseg, float max_norm, void* workspace,
+                            size_t workspace_bytes, float* out, void* stream) {
+  DIRB_CHECK_ARG(segs_host && nseg > 0 && out && workspace && max_norm > 0.f,
+                 "grad_norm_multi: bad arguments (segs_host %p, nseg %d, out %p, workspace %p, max_norm %g)",
+                 (const void*)segs_host, nseg, (void*)out, workspace, (double)max_norm);
+  DIRB_CHECK_ARG(reinterpret_cast<uintptr_t>(workspace) % 8 == 0, "grad_norm_multi: workspace must be 8-byte aligned");
+  if (workspace_bytes < dirb200_grad_norm_multi_workspace_bytes()) {
+    set_error("grad_norm_multi: workspace too small");
+    return DIRB200_ERR_WORKSPACE;
+  }
+  int64_t total_chunks = 0;
+  for (int k = 0; k < nseg; ++k) {
+    const dirb200_grad_segment& s = segs_host[k];
+    DIRB_CHECK_ARG(s.numel == 0 || s.grad, "grad_norm_multi: segment %d has a null pointer", k);
+    DIRB_CHECK_ARG((reinterpret_cast<uintptr_t>(s.grad) & 3) == 0, "grad_norm_multi: segment %d is not 4-byte aligned",
+                   k);
+    DIRB_CHECK_ARG(s.numel >= 0 && (s.numel - 1) / kAdamChunk < INT32_MAX,
+                   "grad_norm_multi: segment %d has numel %lld (0 .. 2^31 chunks of %d)", k, (long long)s.numel,
+                   kAdamChunk);
+    total_chunks += (s.numel + kAdamChunk - 1) / kAdamChunk;
+  }
+  // one grid for every launch of the call, so that CTA b of each launch adds into the same partial
+  int grid = grid1d(total_chunks, 1, 4);
+  if (grid > kClipMaxGrid) grid = kClipMaxGrid;
+  double* partials = reinterpret_cast<double*>(workspace);
+  unsigned int* ticket = reinterpret_cast<unsigned int*>(partials + kClipMaxGrid);
+  GradNormArgs a;
+  a.max_norm = max_norm;
+  // empty segments are skipped; a launch takes up to kAdamMultiMaxSegs non-empty ones whose chunks fit the int prefix
+  int k = 0;
+  bool first = true;
+  do {
+    int ns = 0;
+    int64_t chunks = 0;
+    a.chunk_start[0] = 0;
+    for (; k < nseg && ns < kAdamMultiMaxSegs; ++k) {
+      const int64_t c = (segs_host[k].numel + kAdamChunk - 1) / kAdamChunk;
+      if (c == 0) continue;
+      if (ns > 0 && chunks + c > INT32_MAX) break;
+      a.grad[ns] = segs_host[k].grad;
+      a.numel[ns] = segs_host[k].numel;
+      chunks += c;
+      a.chunk_start[++ns] = (int)chunks;
+    }
+    while (k < nseg && segs_host[k].numel == 0) ++k;     // so that the last launch knows it is the last
+    a.nseg = ns;
+    a.first = first;
+    a.last = k == nseg;
+    grad_norm_multi_kernel<<<grid, 256, 0, as_stream(stream)>>>(a, partials, ticket, out);
+    DIRB_LAUNCHED();
+    first = false;
+  } while (k < nseg);
   return DIRB200_OK;
 }
 

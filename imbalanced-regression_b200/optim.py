@@ -140,15 +140,30 @@ def _bias_corrections(beta1, beta2, step):
     return 1.0 - math.pow(b1, step), math.sqrt(1.0 - math.pow(b2, step))
 
 
+# dirb200_grad_segment (include/dirb200.h): a device pointer and numel
+_GRAD_SEGMENT = np.dtype([('grad', np.uint64), ('numel', np.int64)])
+
+
 class Adam(torch.optim.Optimizer):
     """Drop-in for torch.optim.Adam(params, lr, betas, eps, weight_decay) with coupled L2 weight decay, as
     nyud2-dir/train.py:146 uses it, on any list of CUDA fp32 tensors: one dirb200_adam_step_multi launch per parameter
     group (one per 512 tensors).  As in torch, a parameter whose .grad is None is skipped and its step count does not
     advance; state is kept per parameter ('step' a CPU fp32 scalar tensor, 'exp_avg', 'exp_avg_sq'), so state_dict()
-    has torch's layout and loads into torch.optim.Adam and back.  amsgrad and maximize are refused."""
+    has torch's layout and loads into torch.optim.Adam and back.  amsgrad and maximize are refused.
+
+    max_grad_norm: each step() first takes the 2-norm over the .grad of every parameter of every group
+    (dirb200_grad_norm_multi), as clip_grad_norm_(model.parameters(), max_grad_norm) does before optimizer.step() at
+    sts-b-dir/trainer.py:147-150, and each group's launch (dirb200_adam_step_multi_clipped) multiplies the gradients by
+    min(1, max_grad_norm / (norm + 1e-6)) as it reads them.  Unlike torch, .grad is NOT rewritten: it keeps the
+    unclipped gradient.  A non-finite norm propagates as in torch (error_if_nonfinite=False): an infinite norm gives a
+    coefficient of 0, a NaN norm a NaN one.  No host synchronisation; last_grad_norm() returns the norm of the most
+    recent step as a device tensor.
+
+    Every group is checked (and, with max_grad_norm, that all gradients share one device) before any state is created
+    or any step count advances, so a refused step() leaves the optimizer as it was."""
 
     def __init__(self, params, lr=1e-3, betas=(0.9, 0.999), eps=1e-8, weight_decay=0, amsgrad=False, *,
-                 maximize=False):
+                 maximize=False, max_grad_norm=None):
         if amsgrad:
             raise ValueError("optim.Adam has no amsgrad variant")
         if maximize:
@@ -163,8 +178,38 @@ class Adam(torch.optim.Optimizer):
             raise ValueError(f"Invalid beta parameter at index 1: {betas[1]}")
         if not 0.0 <= weight_decay:
             raise ValueError(f"Invalid weight_decay value: {weight_decay}")
+        if max_grad_norm is not None and not max_grad_norm > 0.0:
+            raise ValueError(f"Invalid max_grad_norm value: {max_grad_norm}")
         super().__init__(params, dict(lr=lr, betas=tuple(betas), eps=eps, weight_decay=weight_decay, amsgrad=False,
                                       maximize=False))
+        # one norm over every group, so the option and its device buffers live on the optimizer, not in a group or in
+        # the per-parameter state (state_dict() stays torch's)
+        self.max_grad_norm = max_grad_norm
+        self._clip_ws = self._clip_out = None
+
+    def last_grad_norm(self):
+        """Norm seen by the most recent clipped step, or None: a device tensor of its own (a device-side copy, no
+        sync), so the next step() does not change it."""
+        return None if self._clip_out is None else self._clip_out[1].clone()
+
+    def _clip_coef(self, groups):
+        """dirb200_grad_norm_multi over the gradients of every prepared group; the device coefficient, or None when
+        there is nothing to clip."""
+        gs = [g for _, gs, _, _ in groups for g in gs]
+        if self.max_grad_norm is None or not gs:
+            return None
+        dev = groups[0][3]
+        if self._clip_out is None or self._clip_out.get_device() != dev:
+            self._clip_ws = torch.zeros(_lib.raw("dirb200_grad_norm_multi_workspace_bytes")(), dtype=torch.uint8,
+                                        device=gs[0].device)
+            self._clip_out = torch.zeros(2, dtype=torch.float32, device=gs[0].device)
+        table = np.empty(len(gs), dtype=_GRAD_SEGMENT)
+        table['grad'] = [g.data_ptr() for g in gs]
+        table['numel'] = [g.numel() for g in gs]
+        with torch.cuda.device(dev):
+            _lib.call("dirb200_grad_norm_multi", table.ctypes.data_as(_lib.P), len(gs), float(self.max_grad_norm),
+                      _lib.ptr(self._clip_ws), self._clip_ws.numel(), _lib.ptr(self._clip_out), _lib.stream_ptr())
+        return self._clip_out[0:1]
 
     @staticmethod
     def _refuse(ps, gs, states):
@@ -191,6 +236,9 @@ class Adam(torch.optim.Optimizer):
         if closure is not None:
             with torch.enable_grad():
                 loss = closure()
+        # every group is checked before any state changes, and every segment table is built before the first launch:
+        # the clipping norm covers them all
+        checked = []
         for group in self.param_groups:
             if group.get('amsgrad') or group.get('maximize') or group.get('decoupled_weight_decay'):
                 raise ValueError("optim.Adam: amsgrad, maximize and decoupled weight decay are not supported")
@@ -199,7 +247,11 @@ class Adam(torch.optim.Optimizer):
                 continue
             gs = [p.grad for p in ps]
             states = [self.state.get(p) for p in ps]
-            dev = self._refuse(ps, gs, states)
+            checked.append((group, ps, gs, states, self._refuse(ps, gs, states)))
+        if self.max_grad_norm is not None and len({dev for *_, dev in checked}) > 1:
+            raise _lib.Dirb200Error("optim.Adam(max_grad_norm): the parameters span more than one device")
+        groups = []
+        for group, ps, gs, states, dev in checked:
             for k, p in enumerate(ps):
                 if not states[k]:
                     st = states[k] = self.state[p]
@@ -209,25 +261,40 @@ class Adam(torch.optim.Optimizer):
             steps = [st['step'] for st in states]
             torch._foreach_add_(steps, 1)
             live = [k for k, p in enumerate(ps) if p.numel() > 0]
-            if not live:
+            table = None
+            if live:
+                table = self._segment_table(group, ps, gs, states, steps, live)
+            groups.append((table, gs, group, dev))
+        clip = self._clip_coef(groups)
+        for table, _, group, dev in groups:
+            if table is None:
                 continue
             b1, b2 = group['betas']
-            table = np.empty(len(live), dtype=_SEGMENT)
-            table['param'] = [ps[k].data_ptr() for k in live]
-            table['grad'] = [gs[k].data_ptr() for k in live]
-            table['exp_avg'] = [states[k]['exp_avg'].data_ptr() for k in live]
-            table['exp_avg_sq'] = [states[k]['exp_avg_sq'].data_ptr() for k in live]
-            table['numel'] = [ps[k].numel() for k in live]
-            bcs = {}
-            for k, t in enumerate(torch.stack([steps[k] for k in live]).tolist()):
-                if t not in bcs:
-                    bcs[t] = _bias_corrections(b1, b2, int(t))
-                table['bc1'][k], table['bc2_sqrt'][k] = bcs[t]
-            args = (table.ctypes.data_as(_lib.P), len(live), float(group['lr']), float(b1), float(b2),
+            args = (table.ctypes.data_as(_lib.P), len(table), float(group['lr']), float(b1), float(b2),
                     float(group['eps']), float(group['weight_decay']))
+            name = "dirb200_adam_step_multi"
+            if clip is not None:
+                name, args = "dirb200_adam_step_multi_clipped", args + (_lib.ptr(clip),)
             if dev == torch.cuda.current_device():
-                _lib.call("dirb200_adam_step_multi", *args, _lib.stream_ptr())
+                _lib.call(name, *args, _lib.stream_ptr())
             else:
                 with torch.cuda.device(dev):
-                    _lib.call("dirb200_adam_step_multi", *args, _lib.stream_ptr())
+                    _lib.call(name, *args, _lib.stream_ptr())
         return loss
+
+    @staticmethod
+    def _segment_table(group, ps, gs, states, steps, live):
+        """dirb200_adam_segment table of the parameters ps[k], k in live, with each one's bias corrections."""
+        b1, b2 = group['betas']
+        table = np.empty(len(live), dtype=_SEGMENT)
+        table['param'] = [ps[k].data_ptr() for k in live]
+        table['grad'] = [gs[k].data_ptr() for k in live]
+        table['exp_avg'] = [states[k]['exp_avg'].data_ptr() for k in live]
+        table['exp_avg_sq'] = [states[k]['exp_avg_sq'].data_ptr() for k in live]
+        table['numel'] = [ps[k].numel() for k in live]
+        bcs = {}
+        for k, t in enumerate(torch.stack([steps[k] for k in live]).tolist()):
+            if t not in bcs:
+                bcs[t] = _bias_corrections(b1, b2, int(t))
+            table['bc1'][k], table['bc2_sqrt'][k] = bcs[t]
+        return table

@@ -57,6 +57,9 @@ _lib.register({
     "dirb200_sgd_step": (c_int, [P, P, P, c_int64, c_float, c_float, c_float, c_int, c_float, P, P]),
     "dirb200_grad_clip_workspace_bytes": (ctypes.c_size_t, []),
     "dirb200_grad_clip_coef": (c_int, [P, c_int64, c_float, c_float, P, ctypes.c_size_t, P, P]),
+    "dirb200_adam_step_multi_clipped": (c_int, [P, c_int, c_float, c_float, c_float, c_float, c_float, P, P]),
+    "dirb200_grad_norm_multi_workspace_bytes": (ctypes.c_size_t, []),
+    "dirb200_grad_norm_multi": (c_int, [P, c_int, c_float, P, ctypes.c_size_t, P, P]),
 })
 
 

@@ -291,6 +291,19 @@ int dirb200_depth_metrics_accumulate(const float* pred, int ph, int pw, const fl
                                      int64_t n_images, int h, int w, const uint8_t* group_of_bin, int nbins,
                                      double* acc, void* workspace, size_t workspace_bytes, void* stream);
 
+/* STS-B-DIR's STSShotAverage.get_metric (replaces sts-b-dir/util.py:123-172, metrics mse / l1 / gmean / pearsonr /
+ * spearmanr as tasks.py:86 asks for them) over n fp32 predictions and labels (n <= 2^22):
+ * out24[g * 6 + k], g = 0 overall, 1 many, 2 medium, 3 few; k = 0 num_samples, 1 MSE, 2 L1, 3 G-mean, 4 Pearson,
+ * 5 Spearman, all fp64 with x = 5 pred.  A label's group is its DIRB200_BIN_EDGES5 bin over 50 bins in util.py:110-113's
+ * table (a negative label: few).  An exact zero difference enters the G-mean as 1e-10; Pearson is scipy's centred
+ * formula clipped to [-1, 1] (rounded at n = 2, NaN for a constant input); Spearman is the Pearson of the average ranks
+ * within the group, found exactly by an O(n^2) pair count; a group of size 0 reports 0 everywhere, one of size 1 0 for
+ * both correlations.  Two launches, no floating-point atomics: identical calls give identical bits.  workspace: 16 n
+ * bytes, 16-byte aligned (none for n = 0). */
+size_t dirb200_stsb_shot_metrics_workspace_bytes(int64_t n);
+int dirb200_stsb_shot_metrics(const float* preds, const float* labels, int64_t n, void* workspace,
+                              size_t workspace_bytes, double* out24, void* stream);
+
 /* ------------------------------------------------- convolution stack ---- */
 /* Activations are NHWC bf16; weights arrive in the reference's fp32
  * [Cout][Cin][KH][KW] layout (agedb-dir/resnet.py:46-51,79,112-118, i.e. the
@@ -522,6 +535,31 @@ typedef struct dirb200_adam_segment {
  * not for others). */
 int dirb200_adam_step_multi(const dirb200_adam_segment* segs_host, int nseg, float lr, float beta1, float beta2,
                             float eps, float weight_decay, void* stream);
+/* The same step with gradient-norm clipping, the replacement of clip_grad_norm(model.parameters(), max_grad_norm)
+ * followed by optimizer.step() at sts-b-dir/trainer.py:147-150 (Adam, weight decay 1e-5, trainer.py:21): every
+ * gradient is multiplied by the device scalar *clip_coef (dirb200_grad_norm_multi's out[0]) as it is read, and the
+ * gradients are not rewritten.  Same kernel and arithmetic as dirb200_adam_step_multi: a coefficient of exactly 1
+ * gives the same bits. */
+int dirb200_adam_step_multi_clipped(const dirb200_adam_segment* segs_host, int nseg, float lr, float beta1,
+                                    float beta2, float eps, float weight_decay, const float* clip_coef, void* stream);
+
+/* One gradient of dirb200_grad_norm_multi: a 4-byte aligned fp32 device buffer of numel >= 0 elements (NULL when
+ * empty). */
+typedef struct dirb200_grad_segment {
+  const float* grad;
+  int64_t numel;
+} dirb200_grad_segment;
+
+/* torch.nn.utils.clip_grad_norm_'s norm and coefficient over a list of gradients (sts-b-dir/trainer.py:147-149,
+ * --max_grad_norm): out[0] = min(1, max_norm / (||g||_2 + 1e-6)) (a NaN norm gives a NaN coefficient, as torch's
+ * clamp), out[1] = ||g||_2 over every element of every segment.  segs_host is a HOST array passed by value in the
+ * kernel parameters, one launch per 512 non-empty segments; the launches add into the workspace's fp64 partials and
+ * the last one finalises.  Squares are summed in fp32 over at most 16 elements per thread, then in fp64; no
+ * floating-point atomics, so two identical calls give identical bits.  The workspace (>= 8 KiB + 16 B, 8-byte
+ * aligned) must be zero-initialised once; the kernel leaves its ticket word reset. */
+size_t dirb200_grad_norm_multi_workspace_bytes(void);
+int dirb200_grad_norm_multi(const dirb200_grad_segment* segs_host, int nseg, float max_norm, void* workspace,
+                            size_t workspace_bytes, float* out, void* stream);
 
 /* torch.nn.utils.clip_grad_norm_ over one flat gradient buffer (sts-b-dir/trainer.py:147-149, --max_grad_norm):
  * out[0] = min(1, max_norm / (||grad_scale * grads||_2 + 1e-6)), out[1] = that norm.  The gradients themselves are

@@ -77,6 +77,10 @@ _SIGS = {
     "dirb200_layer_bn_bwd_apply": (c_int, [P, P, P, P, P, P, P, P, P, c_int64, c_int, c_int, c_int, P, P, P, P]),
     "dirb200_layer_bn_relu_maxpool_fwd": (c_int, [P, P, P, c_int, c_int, c_int, c_int, P, P, P]),
     "dirb200_layer_maxpool_bwd": (c_int, [P, P, P, c_int, c_int, c_int, c_int, P, P]),
+    # test aids: the runner's batched weight re-layout, split-K reduction and eval-BatchNorm kernels
+    "dirb200_prep_weights_all": (c_int, [P, P, c_int, P]),
+    "dirb200_wgrad_reduce_all": (c_int, [P, c_int, P, P]),
+    "dirb200_bn_eval_coeffs_all": (c_int, [P, c_int, P, P, c_float, P]),
     "dirb200_upsample_bilinear_fwd": (c_int, [P, c_int, c_int, c_int, c_int, c_int, c_int, P, P]),
     "dirb200_upsample_bilinear_bwd": (c_int, [P, c_int, c_int, c_int, c_int, c_int, c_int, P, P]),
     "dirb200_copy_channels": (c_int, [P, c_int, c_int, P, c_int, c_int, c_int, c_int64, P]),

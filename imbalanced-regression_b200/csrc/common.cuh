@@ -6,6 +6,7 @@
 #include <stdio.h>
 #include <stdlib.h>
 #include <atomic>
+#include <vector>
 #include "../../include/dirb200.h"
 
 namespace dirb200 {
@@ -86,6 +87,25 @@ inline FastDiv make_fastdiv(uint32_t d) {
   f.mul = static_cast<uint32_t>(((1ull << p) + f.d - 1) / f.d);
   f.shr = p - 32;
   return f;
+}
+
+// Test aids over a HOST array of jobs: the descriptors go to a device table that lives in stream order around the
+// launch (allocated, copied, launched and freed on st); launch(table) returns the launch's rc.
+template <typename Desc, typename Launch>
+static int with_device_table(const std::vector<Desc>& descs, cudaStream_t st, Launch&& launch) {
+  Desc* dev = nullptr;
+  const size_t bytes = sizeof(Desc) * descs.size();
+  DIRB_CUDA(cudaMallocAsync(reinterpret_cast<void**>(&dev), bytes, st));
+  cudaError_t e = cudaMemcpyAsync(dev, descs.data(), bytes, cudaMemcpyHostToDevice, st);
+  int rc = DIRB200_OK;
+  if (e != cudaSuccess) {
+    set_error("cudaMemcpyAsync of a descriptor table -> %s", cudaGetErrorString(e));
+    rc = DIRB200_ERR_CUDA;
+  } else {
+    rc = launch(dev);
+  }
+  DIRB_CUDA(cudaFreeAsync(dev, st));
+  return rc;
 }
 
 // streaming 128-bit global load that does not allocate in L1

@@ -250,6 +250,19 @@ static int to_shape(int n, int h, int w, int cin, int cout, int kh, int kw, int 
   return DIRB200_OK;
 }
 
+/* ---- Test aids: the runner's batched weight re-layout and split-K reduction, one launch over caller-given jobs (see
+ * include/dirb200.h).  The jobs become the runner's own descriptors (make_prep_desc, WgradReduceDesc) in a device table
+ * that lives in stream order around the launch. */
+static int conv_job_shape_ok(const char* who, int k, int cout, int cin, int kh, int kw, int stem) {
+  DIRB_CHECK_ARG(cout > 0 && cin > 0 && kh > 0 && kw > 0, "%s: job %d has a non-positive size (%d, %d, %d, %d)", who, k,
+                 cout, cin, kh, kw);
+  DIRB_CHECK_ARG(!stem || (cin == 3 && kh == 7 && kw == 7), "%s: job %d: the stem must be 3x7x7", who, k);
+  const int64_t weights = (int64_t)cout * cin * kh * kw;
+  DIRB_CHECK_ARG(weights < (int64_t(1) << 31) && (!stem || 256 * (int64_t)cout < (int64_t(1) << 31)),
+                 "%s: job %d has 2^31 or more weights", who, k);
+  return DIRB200_OK;
+}
+
 }  // namespace dirb200
 
 using namespace dirb200;
@@ -364,6 +377,40 @@ int dirb200_conv_plan(int n, int h, int w, int cin, int cout, int kh, int kw, in
   ConvShape s;
   if (int rc = to_shape(n, h, w, cin, cout, kh, kw, stride, pad, stem, &s)) return rc;
   return conv_plan(s, stem != 0, op, plan7);
+}
+
+int dirb200_prep_weights_all(const float* params, const dirb200_prep_job* jobs_host, int njobs, void* stream) {
+  DIRB_CHECK_ARG(params && jobs_host, "prep_weights_all: null pointer");
+  DIRB_CHECK_ARG(njobs >= 1 && njobs <= 65535, "prep_weights_all: njobs must be 1 .. 65535 (got %d)", njobs);
+  std::vector<PrepDesc> descs;
+  for (int k = 0; k < njobs; ++k) {
+    const dirb200_prep_job& j = jobs_host[k];
+    DIRB_CHECK_ARG(j.w_fprop, "prep_weights_all: job %d has a null w_fprop", k);
+    DIRB_CHECK_ARG(j.w_off >= 0, "prep_weights_all: job %d has a negative w_off", k);
+    if (int rc = conv_job_shape_ok("prep_weights_all", k, j.cout, j.cin, j.kh, j.kw, j.stem)) return rc;
+    DIRB_CHECK_ARG(!j.stem || !j.w_dgrad, "prep_weights_all: job %d: the stem has no dgrad operand (w_dgrad must be null)",
+                   k);
+    descs.push_back(make_prep_desc((size_t)j.w_off, j.cout, j.cin, j.kh, j.kw, j.stem ? 1 : 0,
+                                   (__nv_bfloat16*)j.w_fprop, (__nv_bfloat16*)j.w_dgrad));
+  }
+  cudaStream_t st = as_stream(stream);
+  return with_device_table(descs, st, [&](const PrepDesc* d) { return prep_weights_all(params, d, njobs, st); });
+}
+
+int dirb200_wgrad_reduce_all(const dirb200_wgrad_reduce_job* jobs_host, int njobs, float* grads, void* stream) {
+  DIRB_CHECK_ARG(jobs_host && grads, "wgrad_reduce_all: null pointer");
+  DIRB_CHECK_ARG(njobs >= 1 && njobs <= 65535, "wgrad_reduce_all: njobs must be 1 .. 65535 (got %d)", njobs);
+  std::vector<WgradReduceDesc> descs;
+  for (int k = 0; k < njobs; ++k) {
+    const dirb200_wgrad_reduce_job& j = jobs_host[k];
+    DIRB_CHECK_ARG(j.partial, "wgrad_reduce_all: job %d has a null partial", k);
+    DIRB_CHECK_ARG(j.w_off >= 0, "wgrad_reduce_all: job %d has a negative w_off", k);
+    DIRB_CHECK_ARG(j.splits >= 1, "wgrad_reduce_all: job %d: splits must be at least 1 (got %d)", k, j.splits);
+    if (int rc = conv_job_shape_ok("wgrad_reduce_all", k, j.cout, j.cin, j.kh, j.kw, j.stem)) return rc;
+    descs.push_back(WgradReduceDesc{j.partial, (size_t)j.w_off, j.splits, j.cout, j.cin, j.kh, j.kw, j.stem ? 1 : 0});
+  }
+  cudaStream_t st = as_stream(stream);
+  return with_device_table(descs, st, [&](const WgradReduceDesc* d) { return wgrad_reduce_all(d, njobs, grads, st); });
 }
 
 }  // extern "C"

@@ -1429,6 +1429,29 @@ int dirb200_bn_eval_coeffs(int c, const float* gamma, const float* beta, float e
   return bn_eval_coeffs(c, gamma, beta, eps, running_mean, running_var, scale, shift, as_stream(stream));
 }
 
+/* Test aid: the runner's one-launch eval coefficients of every BatchNorm, over caller-given jobs (see include/dirb200.h). */
+int dirb200_bn_eval_coeffs_all(const dirb200_bn_eval_job* jobs_host, int njobs, const float* params,
+                               const float* running, float eps, void* stream) {
+  DIRB_CHECK_ARG(jobs_host && params && running, "bn_eval_coeffs_all: null pointer");
+  DIRB_CHECK_ARG(njobs >= 1 && njobs <= 65535, "bn_eval_coeffs_all: njobs must be 1 .. 65535 (got %d)", njobs);
+  std::vector<BnEvalDesc> descs;
+  int max_c = 0;
+  for (int k = 0; k < njobs; ++k) {
+    const dirb200_bn_eval_job& j = jobs_host[k];
+    DIRB_CHECK_ARG(j.scale && j.shift, "bn_eval_coeffs_all: job %d has a null scale or shift", k);
+    DIRB_CHECK_ARG(j.c > 0, "bn_eval_coeffs_all: job %d has a non-positive channel count %d", k, j.c);
+    DIRB_CHECK_ARG(j.gamma_off >= 0 && j.beta_off >= 0 && j.rm_off >= 0 && j.rv_off >= 0,
+                   "bn_eval_coeffs_all: job %d has a negative offset", k);
+    descs.push_back(BnEvalDesc{j.c, (size_t)j.gamma_off, (size_t)j.beta_off, (size_t)j.rm_off, (size_t)j.rv_off, j.scale,
+                               j.shift});
+    if (j.c > max_c) max_c = j.c;
+  }
+  cudaStream_t st = as_stream(stream);
+  return with_device_table(descs, st, [&](const BnEvalDesc* d) {
+    return bn_eval_coeffs_all(d, njobs, max_c, params, running, eps, st);
+  });
+}
+
 /* ---- Test aids: the consumers of the per-CTA rows the conv epilogues write (see include/dirb200.h). */
 int dirb200_bn_finalize_layout(const float* partial, const int* layout_host, int64_t rows, int c, const float* gamma,
                                const float* beta, float eps, float momentum, float* running_mean, float* running_var,

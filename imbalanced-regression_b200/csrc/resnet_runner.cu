@@ -892,4 +892,43 @@ int dirb200_resnet_peek(dirb200_net* net, int block, int which, void** ptr, int6
   DIRB_CHECK_ARG(*ptr, "resnet_peek: tensor not materialised");
   return DIRB200_OK;
 }
+
+/* Test / debugging aid: one conv layer's buffers, offset, shape and the split factor of its reduction-table entry.
+ * block = -1: stem (conv 0); block >= 0: conv 0 / 1 / 2 / 3 = conv1 / conv2 / conv3 / downsample. */
+int dirb200_resnet_peek_conv(dirb200_net* net, int block, int conv, dirb200_conv_peek* out) {
+  DIRB_CHECK_ARG(net && out, "resnet_peek_conv: null pointer");
+  DIRB_CHECK_ARG(block >= -1 && block < (int)net->blocks.size(), "resnet_peek_conv: bad block %d", block);
+  DIRB_CHECK_ARG(conv >= 0 && conv <= (block < 0 ? 0 : 3), "resnet_peek_conv: bad conv %d", conv);
+  // the reduction table holds the stem, then every block's c1, c2, c3 [, ds] in block order (build())
+  int entry = 0;
+  const ConvLayer* cv = &net->stem;
+  if (block >= 0) {
+    const Block& B = net->blocks[block];
+    DIRB_CHECK_ARG(conv < 3 || B.has_ds, "resnet_peek_conv: block %d has no downsample", block);
+    entry = 1;
+    for (int b = 0; b < block; ++b) entry += net->blocks[b].has_ds ? 4 : 3;
+    entry += conv;
+    const ConvLayer* convs[4] = {&B.c1, &B.c2, &B.c3, &B.ds};
+    cv = convs[conv];
+  }
+  WgradReduceDesc d{};
+  DIRB_CUDA(cudaMemcpy(&d, net->reduce_descs + entry, sizeof(d), cudaMemcpyDeviceToHost));
+  DIRB_CHECK_ARG(d.partial == cv->wpart && d.w_off == cv->w_off,
+                 "resnet_peek_conv: reduction-table entry %d does not belong to this conv", entry);
+  out->w_fprop = cv->wf;
+  out->w_dgrad = cv->wd;
+  out->partial = cv->wpart;
+  out->scale = cv->bn.scale;
+  out->shift = cv->bn.shift;
+  out->w_off = (int64_t)cv->w_off;
+  if (cv->stem) {
+    out->cout = cv->s.cout; out->cin = 3; out->kh = 7; out->kw = 7; out->stride = 2; out->pad = 3;
+  } else {
+    out->cout = cv->s.cout; out->cin = cv->s.cin; out->kh = cv->s.kh; out->kw = cv->s.kw; out->stride = cv->s.stride;
+    out->pad = cv->s.pad;
+  }
+  out->stem = cv->stem ? 1 : 0;
+  out->splits = d.splits;
+  return DIRB200_OK;
+}
 }

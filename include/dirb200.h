@@ -428,6 +428,47 @@ int dirb200_layer_bn_relu_maxpool_fwd(const void* y, const float* scale, const f
 int dirb200_layer_maxpool_bwd(const void* g1, const void* g2, const uint8_t* argmax, int n, int h, int w, int c,
                               void* dx, void* stream);
 
+/* ------------------------------------------------ Test aids: the runner's batched kernels ---- */
+/* The ResNet runner re-lays every conv weight, reduces every conv's split-K weight-gradient partials and forms every
+ * eval-mode BatchNorm's coefficients with ONE launch over a descriptor table each.  These entry points run that launch
+ * once over caller-given jobs, built with the runner's own descriptor construction, so that it can be checked against a
+ * high-precision reference.  jobs_host is a HOST array of 1 .. 65535 jobs; the call copies it to a device table in
+ * stream order (allocated, copied, launched and freed on `stream`).  Every argument is checked on the host before any
+ * CUDA call: null pointers, non-positive sizes, negative offsets, a stem that is not 3x7x7 and a filter of 2^31 or more
+ * weights (the index arithmetic divides 32-bit indices by multiply-high reciprocals) are refused. */
+
+/* One conv: fp32 [cout][cin][kh][kw] at params + w_off -> w_fprop bf16 [cout][kh][kw][cin] and, when w_dgrad is not
+ * NULL, w_dgrad bf16 [cin][kh][kw][cout] (round to nearest even).  stem (cin = 3, 7x7): w_fprop bf16 [cout][256] as
+ * dirb200_conv_prep_weights(stem = 1) forms it; w_dgrad must be NULL. */
+typedef struct dirb200_prep_job {
+  int64_t w_off;
+  int cout, cin, kh, kw, stem;
+  void* w_fprop;
+  void* w_dgrad;
+} dirb200_prep_job;
+int dirb200_prep_weights_all(const float* params, const dirb200_prep_job* jobs_host, int njobs, void* stream);
+
+/* One conv: grads[w_off ..] fp32 [cout][cin][kh][kw] += sum over `splits` of the partials [splits][cout][kh*kw*cin]
+ * (k = (r*kw + s)*cin + c, as the wgrad GEMM writes them); stem (cin = 3, 7x7): partials [splits][cout][256] over the
+ * space-to-depth taps, the padding channel and the taps outside the 7x7 filter dropped. */
+typedef struct dirb200_wgrad_reduce_job {
+  const float* partial;
+  int64_t w_off;
+  int splits, cout, cin, kh, kw, stem;
+} dirb200_wgrad_reduce_job;
+int dirb200_wgrad_reduce_all(const dirb200_wgrad_reduce_job* jobs_host, int njobs, float* grads, void* stream);
+
+/* One BatchNorm of c channels: scale = gamma * rsqrt(running_var + eps), shift = beta - running_mean * scale (fp32 [c]),
+ * gamma / beta at params + gamma_off / beta_off, running_mean / running_var at running + rm_off / rv_off. */
+typedef struct dirb200_bn_eval_job {
+  int c;
+  int64_t gamma_off, beta_off, rm_off, rv_off;
+  float* scale;
+  float* shift;
+} dirb200_bn_eval_job;
+int dirb200_bn_eval_coeffs_all(const dirb200_bn_eval_job* jobs_host, int njobs, const float* params,
+                               const float* running, float eps, void* stream);
+
 /* ------------------------------------------------ ResNet backbone runner ---- */
 /* Opaque native runner of the bottleneck ResNet of agedb-dir/resnet.py:41-70,
  * 73-138 (conv1/bn1/relu/maxpool, layer1-4, avgpool, view) for one fixed
@@ -494,6 +535,23 @@ int dirb200_resnet_read_profile(dirb200_net* net, double* ms_by_kind, int64_t* g
  * block = -1: stem (0 = conv1 raw, 1 = relu(bn1), 6 = max-pool output); block >= 0: 0/1 = conv1 raw / act,
  * 2/3 = conv2 raw / act, 4 = conv3 raw, 5 = downsample raw, 6 = block output. */
 int dirb200_resnet_peek(dirb200_net* net, int block, int which, void** ptr, int64_t* rows, int* channels);
+
+/* Test / debugging aid: one conv layer's own buffers and descriptor entries.  block = -1: the stem (conv 0);
+ * block >= 0: conv 0 / 1 / 2 / 3 = conv1 / conv2 / conv3 / downsample.  w_fprop / w_dgrad: its bf16 GEMM operands
+ * (w_dgrad NULL for the stem); partial: its split-K weight-gradient partials [splits][cout][kh*kw*cin] (stem:
+ * [splits][cout][256]); scale / shift: its BatchNorm's fp32 [cout] coefficients; w_off: its weight's offset in the flat
+ * parameter buffer; cout .. pad: the conv's hyper-parameters (stem: 3 -> cout, 7x7, stride 2, pad 3); splits: the
+ * factor its entry in the runner's split-K reduction table holds (read back from the device: synchronises). */
+typedef struct dirb200_conv_peek {
+  void* w_fprop;
+  void* w_dgrad;
+  float* partial;
+  float* scale;
+  float* shift;
+  int64_t w_off;
+  int cout, cin, kh, kw, stride, pad, stem, splits;
+} dirb200_conv_peek;
+int dirb200_resnet_peek_conv(dirb200_net* net, int block, int conv, dirb200_conv_peek* out);
 
 /* nn.Linear(feature_dim, 1) (resnet.py:88,148): pred[n] = x[n,d] . w[d] + bias */
 int dirb200_linear1_fwd(const float* x, const float* w, const float* bias, int64_t n, int d, float* pred,

@@ -135,6 +135,19 @@ def test_conv_forms(cfg):
     run_conv(*cfg)
 
 
+@pytest.mark.parametrize("cfg,device_rng", [
+    # the BiLSTM's GEMMs (imbalanced-regression_b200/rnn.py) as the 1x1 convs over an n = 1, h = T, w = M "image" they
+    # run as: Cout = 8 Hp gate columns (both directions), K = T M = 10 240 pixels in wgrad
+    ((1, 40, 256, 320, 12288, 1, 1, 0), True),    # layer 0's projection, W_ih wgrad, dx: d_word 300 pads to 320, so
+                                                  # dgrad's N = 320 runs in 64-wide tiles
+    ((1, 40, 256, 3072, 12288, 1, 1, 0), True),   # layer 1 (input 2 Hp = 3072)
+    ((1, 40, 256, 1536, 6144, 1, 1, 0), True),    # the W_hh wgrad of one direction (K = Hp, N = 4 Hp)
+    ((1, 9, 10, 64, 512, 1, 1, 0), False),        # the small model (H 20, T 9, M 10): 90 pixels, a ragged k-block
+], ids=["lstm-l0", "lstm-l1", "lstm-whh", "lstm-small"])
+def test_conv_lstm_forms(cfg, device_rng):
+    run_conv(*cfg, seed=4, device_rng=device_rng)
+
+
 def test_conv_layer1_full_batch_shape():
     # a BASELINE-size layer: batch 32 of the 56x56x64 3x3 (M = 100 352 rows, 784 tiles)
     run_conv(32, 56, 56, 64, 64, 3, 1, 1, seed=1)

@@ -11,6 +11,10 @@ Bounds:
 - Recurrent backward step: dh = dgates' . W_hh + dy with the same GEMM bound (K = 4Hp).  The cell backward is a few
   fp32 products of values in [-1, 1] times dh / dc (relative 2^-20 each), then rounding to bf16: relative 2^-8 plus
   (e_dh + 2^-20 |dc|) times the gate factors.
+- Whole layer backward (dirb200_lstm_layer_bwd): the steps are deterministic, so the layer must give the bits of its
+  steps launched one at a time for s = T-1 .. 0; each step is then held to the step bound above given the dg[s + 1] and
+  dc it read (teacher forcing, so errors do not compound through the bound).
+- Inference forward (save = 0): the same arithmetic as save = 1 on two ping-pong state slots, so the same bits.
 - Max-pool and pair features: the maximum of fp32 products is exact, so u and v equal torch's max in fp32 bit for bit,
   and the backward scatter is one fp32 expression rounded to bf16, equal to the same expression in torch.
 - The whole model (no teacher forcing): the native error must be within 8 x the difference between the float64 oracle
@@ -48,14 +52,14 @@ def gate_perm(H, Hp):
     return torch.where(u < H, g * H + u, torch.full_like(n, -1))
 
 
-def prep(H, din, blocks, Dp, seed):
+def prep(H, din, blocks, Dp, seed, scale=0.3):
     import _lib
     g = torch.Generator().manual_seed(seed)
     Hp = pad64(H)
     w = []
     for _ in range(2):
-        w += [torch.randn(4 * H, din, generator=g) * 0.3, torch.randn(4 * H, H, generator=g) * 0.3,
-              torch.randn(4 * H, generator=g) * 0.3, torch.randn(4 * H, generator=g) * 0.3]
+        w += [torch.randn(4 * H, din, generator=g) * scale, torch.randn(4 * H, H, generator=g) * scale,
+              torch.randn(4 * H, generator=g) * scale, torch.randn(4 * H, generator=g) * scale]
     w = [t.to(_dev()) for t in w]
     out = [torch.full((8 * Hp, Dp), float("nan"), dtype=torch.bfloat16, device=_dev()),
            torch.full((Dp, 8 * Hp), float("nan"), dtype=torch.bfloat16, device=_dev()),
@@ -261,9 +265,19 @@ def test_bwd_step_one_launch(H, M, s):
         dc[:, (s + 1) & 1] = torch.randn(2, M, Hp, device=_dev(), generator=g)
         dc[:, (s + 1) & 1][:, ~act_next] = 0
         dc[..., H:] = 0
+    dc_in = dc[:, (s + 1) & 1].clone()
     _lib.call("dirb200_lstm_bwd_step", _lib.ptr(whhT), _lib.ptr(dy), _lib.ptr(gates), _lib.ptr(c), _lib.ptr(lens), T,
               M, Hp, s, _lib.ptr(dc), _lib.ptr(dg), _lib.ptr(dgt), None)
     torch.cuda.synchronize()
+    _check_bwd_step(whhT, dy, gates, c, lens, dg, dgt, dc_in if s + 1 < T else None, dc[:, s & 1], s, H)
+
+
+def _check_bwd_step(whhT, dy, gates, c, lens, dg, dgt, dc_in, dc_out, s, H):
+    """Step s's outputs (dg[:, s], its time-order copy in dgt, the carried dc) against float64 from what the step read
+    (dg[:, s + 1] and dc_in, the dc slot (s + 1) & 1 before the step; None at s = T - 1), within the bounds of the
+    module docstring.  Inert rows and padded units get exact zeros."""
+    T, M, Hp = dg.shape[1], dg.shape[2], whhT.shape[1]
+    perm = gate_perm(H, Hp).to(_dev())
     rows = torch.arange(M, device=_dev())
     active = s < lens.long()
     for d in range(2):
@@ -273,7 +287,7 @@ def test_bwd_step_one_launch(H, M, s):
             W = whhT[d].double()
             dh = A @ W.t()
             edh = (4 * Hp + 4) * U * (A.abs() @ W.abs().t())
-            dcn = dc[d, (s + 1) & 1].double()
+            dcn = dc_in[d].double()
         else:
             dh = torch.zeros(M, Hp, dtype=torch.float64, device=_dev())
             edh = torch.zeros_like(dh)
@@ -297,10 +311,118 @@ def test_bwd_step_one_launch(H, M, s):
         assert torch.all(got.view(M, 4 * Hp)[:, perm < 0] == 0)
         gt = dgt[tau, rows, d * 4 * Hp:(d + 1) * 4 * Hp]
         assert torch.equal(gt, dg[d, s])
-        dcp = dc[d, s & 1].double().view(sh)
+        dcp = dc_out[d].double().view(sh)
         edc = (edh + 2.0 ** -19 * (dh.abs() + dcn.abs() + 1)) * (1 + cp.abs())
-        assert torch.all(~active[:, None, None] | ((dcp - dct * f).abs() <= edc))
+        assert torch.all(~active[:, None, None] | ((dcp - dct * f).abs() <= edc)), (d, s)
         assert torch.all(active[:, None, None] | (dcp == 0))
+        assert torch.all(dc_out[d, :, H:] == 0)
+
+
+def _same_bits(a, b):
+    """Bit-for-bit equality, NaN fill included."""
+    it = {2: torch.int16, 4: torch.int32}[a.element_size()]
+    return a.dtype == b.dtype and a.shape == b.shape and torch.equal(a.view(it), b.view(it))
+
+
+def _layer_fwd(T, M, H, seed):
+    """dirb200_lstm_layer_fwd (save = 1) on random xproj (zero at padded gate columns) and weights at torch's init
+    scale 1 / sqrt(H), so the gates and cells are those of a working layer rather than saturated ones.  Every output
+    buffer is prefilled with NaN (gates stay NaN at inert rows).  Returns (whh, whhT, bias), lens and
+    (xproj, h, c, gates, y)."""
+    import _lib
+    Hp = pad64(H)
+    _, (_, _, whh, whhT, bias) = prep(H, 64, 1, 64, seed, scale=H ** -0.5)
+    perm = gate_perm(H, Hp).to(_dev())
+    lens = lens_for(M, T, seed + 1).to(_dev())
+    g = torch.Generator(device=_dev()).manual_seed(seed + 2)
+    xproj = torch.randn(T, M, 2, 4 * Hp, device=_dev(), generator=g).bfloat16()
+    xproj[..., perm < 0] = 0
+    nan = float("nan")
+    h = torch.full((2, T + 1, M, Hp), nan, dtype=torch.bfloat16, device=_dev())
+    c = torch.full((2, T + 1, M, Hp), nan, device=_dev())
+    gates = torch.full((2, T, M, 4 * Hp), nan, device=_dev())
+    y = torch.full((T, M, 2 * Hp), nan, dtype=torch.bfloat16, device=_dev())
+    _lib.call("dirb200_lstm_layer_fwd", _lib.ptr(xproj), _lib.ptr(whh), _lib.ptr(bias), _lib.ptr(lens), T, M, Hp, 1,
+              _lib.ptr(h), _lib.ptr(c), _lib.ptr(gates), _lib.ptr(y), None)
+    return (whh, whhT, bias), lens, (xproj, h, c, gates, y)
+
+
+def _layer_bwd_teacher_forced(T, M, H, seed):
+    """dirb200_lstm_layer_bwd (s = T-1 .. 0 in one call) on gates and c from a native forward and a random bf16 dy
+    (zero at padded units and at t >= len):
+    - its dg, dg_time and final two-slot dc equal those of dirb200_lstm_bwd_step run for s = T-1 .. 0 on fresh NaN
+      buffers, bit for bit (the step order, the range of s, the dc carry);
+    - every step is within _check_bwd_step's bound, given the dg[s + 1] and dc slot it read;
+    - dg and dg_time are written everywhere, dg_time exactly zero at t >= len and at padded gate columns."""
+    import _lib
+    Hp = pad64(H)
+    (_, whhT, _), lens, (_, h, c, gates, _) = _layer_fwd(T, M, H, seed)
+    perm = gate_perm(H, Hp).to(_dev())
+    mask = torch.arange(T, device=_dev())[:, None] < lens.long()[None, :]        # [T, M]: t < len
+    g = torch.Generator(device=_dev()).manual_seed(seed + 3)
+    dy = torch.randn(T, M, 2, Hp, device=_dev(), generator=g).bfloat16()
+    dy[..., H:] = 0
+    dy[~mask] = 0
+    dy = dy.view(T, M, 2 * Hp)
+
+    def bufs():
+        nan = float("nan")
+        return (torch.full((2, 2, M, Hp), nan, device=_dev()),
+                torch.full((2, T, M, 4 * Hp), nan, dtype=torch.bfloat16, device=_dev()),
+                torch.full((T, M, 8 * Hp), nan, dtype=torch.bfloat16, device=_dev()))
+
+    common = (_lib.ptr(whhT), _lib.ptr(dy), _lib.ptr(gates), _lib.ptr(c), _lib.ptr(lens), T, M, Hp)
+    dc, dg, dgt = bufs()
+    _lib.call("dirb200_lstm_layer_bwd", *common, _lib.ptr(dc), _lib.ptr(dg), _lib.ptr(dgt), None)
+    dc1, dg1, dgt1 = bufs()
+    dcs = {}
+    for s in reversed(range(T)):
+        _lib.call("dirb200_lstm_bwd_step", *common, s, _lib.ptr(dc1), _lib.ptr(dg1), _lib.ptr(dgt1), None)
+        dcs[s] = dc1.clone()
+    torch.cuda.synchronize()
+    assert _same_bits(dg, dg1) and _same_bits(dgt, dgt1) and _same_bits(dc, dc1)
+    for s in range(T):
+        _check_bwd_step(whhT, dy, gates, c, lens, dg1, dgt1, dcs[s + 1][:, (s + 1) & 1] if s + 1 < T else None,
+                        dcs[s][:, s & 1], s, H)
+    assert not torch.isnan(dg.float()).any() and not torch.isnan(dgt.float()).any()
+    d4 = dgt.view(T, M, 2, 4 * Hp)
+    assert torch.all(d4[~mask] == 0) and torch.all(d4[..., perm < 0] == 0)
+
+
+def test_layer_bwd_teacher_forced_full_size():
+    _layer_bwd_teacher_forced(40, 256, 1500, 16)
+
+
+@pytest.mark.parametrize("T,M,H", [(1, 10, 20), (6, 1, 20), (7, 130, 100), (5, 33, 64)],
+                         ids=["T1", "M1", "M130-H100", "H64"])
+def test_layer_bwd_teacher_forced_small(T, M, H):
+    """T = 1 (no recurrent product, one dc slot never written), a single row, two row tiles with a ragged second, and
+    H = 64 (no padded unit)."""
+    _layer_bwd_teacher_forced(T, M, H, 17)
+
+
+@pytest.mark.parametrize("T,M,H", [(40, 256, 1500), (39, 256, 1500), (7, 10, 20), (8, 10, 20)],
+                         ids=["full-even", "full-odd", "small-odd", "small-even"])
+def test_layer_fwd_inference_equals_saved(T, M, H):
+    """save = 0 (two ping-pong h / c slots, no gates) gives the save = 1 output bit for bit; its slots end holding the
+    saved run's slots T and T - 1, each at its own parity; a gates buffer passed in is not touched."""
+    import _lib
+    (whh, _, bias), lens, (xproj, h, c, gates, y) = _layer_fwd(T, M, H, 18)
+    Hp = pad64(H)
+    nan = float("nan")
+    h2 = torch.full((2, 2, M, Hp), nan, dtype=torch.bfloat16, device=_dev())
+    c2 = torch.full((2, 2, M, Hp), nan, device=_dev())
+    gates2 = torch.full_like(gates, nan)
+    y2 = torch.full_like(y, nan)
+    _lib.call("dirb200_lstm_layer_fwd", _lib.ptr(xproj), _lib.ptr(whh), _lib.ptr(bias), _lib.ptr(lens), T, M, Hp, 0,
+              _lib.ptr(h2), _lib.ptr(c2), _lib.ptr(gates2), _lib.ptr(y2), None)
+    torch.cuda.synchronize()
+    assert not torch.isnan(y.float()).any()
+    assert _same_bits(y2, y)
+    for p in range(2):
+        slot = T if T % 2 == p else T - 1
+        assert _same_bits(h2[:, p], h[:, slot]) and _same_bits(c2[:, p], c[:, slot]), p
+    assert torch.isnan(gates2).all()
 
 
 def test_col_sum_deterministic_and_exact_order():

@@ -168,6 +168,16 @@ def test_refusals_before_cuda():
     assert raw("dirb200_lstm_layer_fwd")(p, p, p, p, 4, 2, 64, 1, p, p, None, p, None) == -1
     assert "gates" in _lib.last_error()
     assert raw("dirb200_lstm_bwd_step")(p, p, p, p, p, 4, 0, 64, 0, p, p, p, None) == -1
+    # the whole-layer backward: every pointer, then T, M and Hp
+    for k in range(8):
+        args = [p] * 8
+        args[k] = None
+        assert raw("dirb200_lstm_layer_bwd")(*args[:5], 4, 2, 64, *args[5:], None) == -1, k
+        assert "lstm_layer_bwd: null" in _lib.last_error()
+    for T, M, Hp, what in [(0, 2, 64, "T must be"), (4097, 2, 64, "T must be"), (4, 0, 64, "M must be"),
+                           (4, 65536, 64, "M must be"), (4, 2, 0, "Hp"), (4, 2, 100, "Hp"), (4, 2, 4160, "Hp")]:
+        assert raw("dirb200_lstm_layer_bwd")(p, p, p, p, p, T, M, Hp, p, p, p, None) == -1, (T, M, Hp)
+        assert what in _lib.last_error() and "lstm_layer_bwd" in _lib.last_error()
     assert raw("dirb200_pair_maxpool_fwd")(p, p, None, 2, 0, 20, 64, p, p, None) == -1
     assert raw("dirb200_embed_gather")(p, p, p, None, 37, 4, 3, 24, 32, p, None) == -1
     assert raw("dirb200_lstm_prep_weights")(p, p, p, p, p, p, p, p, 20, 24, 3, 64, 64, p, p, p, p, p, None) == -1

@@ -860,16 +860,29 @@ int dirb200_resnet_backward(dirb200_net* net, const float* d_enc, const float* p
 
 extern "C" {
 /* Test / debugging aid: device pointer and shape of an internal activation.
- * block = -1: stem (which 0 = conv1 raw, 1 = relu(bn1), 6 = max-pool output);
- * block >= 0: which 0/1 = conv1 raw / act, 2/3 = conv2 raw / act, 4 = conv3 raw, 5 = downsample raw, 6 = block output. */
+ * block = -1: stem (which 0 = conv1 raw, 1 = relu(bn1), 6 = max-pool output, 7 = max-pool argmax);
+ * block >= 0: which 0/1 = conv1 raw / act, 2/3 = conv2 raw / act, 4 = conv3 raw, 5 = downsample raw, 6 = block output,
+ * 7 = the block output's ReLU mask.  Selectors 7 report bytes: *channels is the row length in bytes. */
 int dirb200_resnet_peek(dirb200_net* net, int block, int which, void** ptr, int64_t* rows, int* channels) {
+  // the selector is checked before the net is dereferenced
+  DIRB_CHECK_ARG(which >= 0 && which <= 7, "resnet_peek: bad selector %d", which);
+  DIRB_CHECK_ARG(block != -1 || which <= 1 || which >= 6, "resnet_peek: bad selector %d for the stem", which);
   DIRB_CHECK_ARG(net && ptr && rows && channels, "resnet_peek: null pointer");
   DIRB_CHECK_ARG(block >= -1 && block < (int)net->blocks.size(), "resnet_peek: bad block %d", block);
   const ConvLayer* cv = nullptr;
   bool act = false;
+  if (which == 7 && block >= 0) {
+    // only a training-mode forward writes the masks (the backward pass reads them); after any other they are stale
+    DIRB_CHECK_ARG(net->forward_was_training,
+                   "resnet_peek: block ReLU mask not materialised (written by a training-mode forward only)");
+    const Block& B = net->blocks[block];
+    *ptr = B.mask; *rows = B.c3.rows; *channels = B.c3.s.cout / 8;
+    return DIRB200_OK;
+  }
   if (block < 0) {
-    if (which == 6) {
-      *ptr = net->pool_out; *rows = (int64_t)net->n * net->pool_h * net->pool_w; *channels = 64;
+    const int64_t pool_rows = (int64_t)net->n * net->pool_h * net->pool_w;
+    if (which == 6 || which == 7) {
+      *ptr = which == 6 ? (void*)net->pool_out : (void*)net->pool_idx; *rows = pool_rows; *channels = 64;
       return DIRB200_OK;
     }
     cv = &net->stem; act = which == 1;
@@ -895,22 +908,33 @@ int dirb200_resnet_peek(dirb200_net* net, int block, int which, void** ptr, int6
 
 /* Test / debugging aid: one conv layer's buffers, offset, shape and the split factor of its reduction-table entry.
  * block = -1: stem (conv 0); block >= 0: conv 0 / 1 / 2 / 3 = conv1 / conv2 / conv3 / downsample. */
-int dirb200_resnet_peek_conv(dirb200_net* net, int block, int conv, dirb200_conv_peek* out) {
-  DIRB_CHECK_ARG(net && out, "resnet_peek_conv: null pointer");
-  DIRB_CHECK_ARG(block >= -1 && block < (int)net->blocks.size(), "resnet_peek_conv: bad block %d", block);
-  DIRB_CHECK_ARG(conv >= 0 && conv <= (block < 0 ? 0 : 3), "resnet_peek_conv: bad conv %d", conv);
+// The conv layer (block, conv) names and its entry in the split-K reduction table; `who` prefixes the refusals.
+static int find_conv(const dirb200_net* net, int block, int conv, const char* who, const ConvLayer** cv_out,
+                     int* entry_out) {
+  DIRB_CHECK_ARG(block >= -1 && block < (int)net->blocks.size(), "%s: bad block %d", who, block);
+  DIRB_CHECK_ARG(conv >= 0 && conv <= (block < 0 ? 0 : 3), "%s: bad conv %d", who, conv);
   // the reduction table holds the stem, then every block's c1, c2, c3 [, ds] in block order (build())
   int entry = 0;
   const ConvLayer* cv = &net->stem;
   if (block >= 0) {
     const Block& B = net->blocks[block];
-    DIRB_CHECK_ARG(conv < 3 || B.has_ds, "resnet_peek_conv: block %d has no downsample", block);
+    DIRB_CHECK_ARG(conv < 3 || B.has_ds, "%s: block %d has no downsample", who, block);
     entry = 1;
     for (int b = 0; b < block; ++b) entry += net->blocks[b].has_ds ? 4 : 3;
     entry += conv;
     const ConvLayer* convs[4] = {&B.c1, &B.c2, &B.c3, &B.ds};
     cv = convs[conv];
   }
+  *cv_out = cv;
+  *entry_out = entry;
+  return DIRB200_OK;
+}
+
+int dirb200_resnet_peek_conv(dirb200_net* net, int block, int conv, dirb200_conv_peek* out) {
+  DIRB_CHECK_ARG(net && out, "resnet_peek_conv: null pointer");
+  int entry = 0;
+  const ConvLayer* cv = nullptr;
+  RUN(find_conv(net, block, conv, "resnet_peek_conv", &cv, &entry));
   WgradReduceDesc d{};
   DIRB_CUDA(cudaMemcpy(&d, net->reduce_descs + entry, sizeof(d), cudaMemcpyDeviceToHost));
   DIRB_CHECK_ARG(d.partial == cv->wpart && d.w_off == cv->w_off,
@@ -929,6 +953,18 @@ int dirb200_resnet_peek_conv(dirb200_net* net, int block, int conv, dirb200_conv
   }
   out->stem = cv->stem ? 1 : 0;
   out->splits = d.splits;
+  return DIRB200_OK;
+}
+
+/* Test / debugging aid: one conv's BatchNorm batch statistics (fp32 [cout] mean, invstd) of the last training-mode
+ * forward.  block / conv as dirb200_resnet_peek_conv. */
+int dirb200_resnet_peek_bn_stats(dirb200_net* net, int block, int conv, float** mean, float** invstd) {
+  DIRB_CHECK_ARG(net && mean && invstd, "resnet_peek_bn_stats: null pointer");
+  int entry = 0;
+  const ConvLayer* cv = nullptr;
+  RUN(find_conv(net, block, conv, "resnet_peek_bn_stats", &cv, &entry));
+  *mean = cv->bn.mean;
+  *invstd = cv->bn.invstd;
   return DIRB200_OK;
 }
 }

@@ -532,8 +532,11 @@ int dirb200_resnet_set_profiling(dirb200_net* net, int enabled);
 int dirb200_resnet_read_profile(dirb200_net* net, double* ms_by_kind, int64_t* groups_by_kind);
 
 /* Test / debugging aid: device pointer + shape ([rows][channels] bf16, NHWC) of an internal activation.
- * block = -1: stem (0 = conv1 raw, 1 = relu(bn1), 6 = max-pool output); block >= 0: 0/1 = conv1 raw / act,
- * 2/3 = conv2 raw / act, 4 = conv3 raw, 5 = downsample raw, 6 = block output. */
+ * block = -1: stem (0 = conv1 raw, 1 = relu(bn1), 6 = max-pool output, 7 = max-pool argmax: u8 [rows][64], r*3 + s of
+ * the window's first maximum); block >= 0: 0/1 = conv1 raw / act, 2/3 = conv2 raw / act, 4 = conv3 raw,
+ * 5 = downsample raw, 6 = block output, 7 = the block output's ReLU mask: [rows][channels] bytes with
+ * channels = C / 8, bit j of byte g = (output channel 8g + j > 0); refused unless the last forward was a training one.
+ * A selector outside 0 .. 7, or 2 .. 5 for the stem, is refused before net is read. */
 int dirb200_resnet_peek(dirb200_net* net, int block, int which, void** ptr, int64_t* rows, int* channels);
 
 /* Test / debugging aid: one conv layer's own buffers and descriptor entries.  block = -1: the stem (conv 0);
@@ -552,6 +555,10 @@ typedef struct dirb200_conv_peek {
   int cout, cin, kh, kw, stride, pad, stem, splits;
 } dirb200_conv_peek;
 int dirb200_resnet_peek_conv(dirb200_net* net, int block, int conv, dirb200_conv_peek* out);
+
+/* Test / debugging aid: the same conv's BatchNorm batch statistics, fp32 [cout] mean and invstd, as the last
+ * training-mode forward left them (its own entry point: dirb200_conv_peek keeps its layout, which callers allocate). */
+int dirb200_resnet_peek_bn_stats(dirb200_net* net, int block, int conv, float** mean, float** invstd);
 
 /* nn.Linear(feature_dim, 1) (resnet.py:88,148): pred[n] = x[n,d] . w[d] + bias */
 int dirb200_linear1_fwd(const float* x, const float* w, const float* bias, int64_t n, int d, float* pred,

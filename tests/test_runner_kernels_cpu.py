@@ -149,3 +149,27 @@ def test_peek_conv_refuses_a_null_net_or_output():
     for block, conv in ((-1, 0), (0, 0), (0, 3)):
         refused("dirb200_resnet_peek_conv", None, block, conv, ctypes.byref(out), msg="null")
     refused("dirb200_resnet_peek_conv", D, 0, 0, None, msg="null")
+
+
+def test_peek_bn_stats_refuses_a_null_net_or_output():
+    import resnet  # noqa: F401  (registers the runner bindings)
+    p = ctypes.c_void_p()
+    for block, conv in ((-1, 0), (0, 0), (0, 3)):
+        refused("dirb200_resnet_peek_bn_stats", None, block, conv, ctypes.byref(p), ctypes.byref(p), msg="null")
+        refused("dirb200_resnet_peek_bn_stats", D, block, conv, None, ctypes.byref(p), msg="null")
+        refused("dirb200_resnet_peek_bn_stats", D, block, conv, ctypes.byref(p), None, msg="null")
+
+
+def test_peek_refuses_bad_selectors_before_reading_the_net():
+    """dirb200_resnet_peek checks its selector before it reads the net (the null net here would otherwise be
+    refused as a null pointer): 0 .. 7 for a block, 0, 1, 6 and 7 for the stem."""
+    import resnet  # noqa: F401  (registers the runner bindings)
+    ptr, rows, ch = ctypes.c_void_p(), ctypes.c_int64(), ctypes.c_int()
+    out = (ctypes.byref(ptr), ctypes.byref(rows), ctypes.byref(ch))
+    for block, which in ((0, 8), (0, -1), (-1, 8), (3, 100), (-1, -2)):
+        refused("dirb200_resnet_peek", None, block, which, *out, msg=f"bad selector {which}")
+    for which in (2, 3, 4, 5):
+        refused("dirb200_resnet_peek", None, -1, which, *out, msg="for the stem")
+    for block, which in ((-1, 0), (-1, 7), (0, 6), (0, 7)):
+        refused("dirb200_resnet_peek", None, block, which, *out, msg="null")
+        refused("dirb200_resnet_peek", D, block, which, None, ctypes.byref(rows), ctypes.byref(ch), msg="null")

@@ -24,16 +24,25 @@ __global__ void prep_weights_kernel(const float* __restrict__ w, int cout, int c
   }
 }
 
-// stem: fp32 [Cout][3][7][7] -> bf16 [Cout][4 r'][4 s'][16 = (ph, pw, c4)], the 7x7/2 conv seen as a 4x4/1 conv
-// over the space-to-depth input; original tap r = 2 r' + ph - 1 (r' = 0, ph = 0 has no tap -> 0).
+// The stem's GEMM sees the 7x7/2 conv as a 4x4/1 conv over the space-to-depth input: its operand index
+// k = (r', s', ph, pw, c4) in [0, 256) is channel c = c4 of the original tap (r, s) = (2 r' + ph - 1, 2 s' + pw - 1).
+// false where k holds no weight: c4 == 3 is padding, and r' = 0 with ph = 0 (likewise s', pw) has no tap.
+__host__ __device__ __forceinline__ bool stem_tap(int k, int& c, int& r, int& s) {
+  const int rp = k >> 6, sp = (k >> 4) & 3, ph = (k >> 3) & 1, pw = (k >> 2) & 1;
+  c = k & 3;
+  r = 2 * rp + ph - 1;
+  s = 2 * sp + pw - 1;
+  return c < 3 && r >= 0 && s >= 0;
+}
+
+// stem: fp32 [Cout][3][7][7] -> bf16 [Cout][4 r'][4 s'][16 = (ph, pw, c4)] (no tap -> 0)
 __global__ void prep_stem_weights_kernel(const float* __restrict__ w, int cout, __nv_bfloat16* __restrict__ wf) {
   const int total = cout * 256;
   for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < total; i += gridDim.x * blockDim.x) {
-    const int co = i >> 8, k = i & 255;
-    const int rp = k >> 6, sp = (k >> 4) & 3, ph = (k >> 3) & 1, pw = (k >> 2) & 1, c = k & 3;
-    const int r = 2 * rp + ph - 1, s = 2 * sp + pw - 1;
+    const int co = i >> 8;
+    int c, r, s;
     float v = 0.f;
-    if (c < 3 && r >= 0 && s >= 0 && r < 7 && s < 7) v = w[((co * 3 + c) * 7 + r) * 7 + s];
+    if (stem_tap(i & 255, c, r, s)) v = w[((co * 3 + c) * 7 + r) * 7 + s];
     wf[i] = __float2bfloat16_rn(v);
   }
 }
@@ -86,10 +95,9 @@ __global__ void wgrad_reduce_stem_kernel(const float* __restrict__ partial, int 
                                          float* __restrict__ dw) {
   const int total = 256 * cout;                   // partial[split][co][k], k = (r', s', ph, pw, c4)
   for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < total; i += gridDim.x * blockDim.x) {
-    const int co = i >> 8, k = i & 255;
-    const int rp = k >> 6, sp_ = (k >> 4) & 3, ph = (k >> 3) & 1, pw = (k >> 2) & 1, c = k & 3;
-    const int r = 2 * rp + ph - 1, s = 2 * sp_ + pw - 1;
-    if (c >= 3 || r < 0 || s < 0) continue;
+    const int co = i >> 8;
+    int c, r, s;
+    if (!stem_tap(i & 255, c, r, s)) continue;
     float acc = 0.f;
     for (int sp = 0; sp < splits; ++sp) acc += partial[(int64_t)sp * total + i];
     float* o = dw + ((co * 3 + c) * 7 + r) * 7 + s;
@@ -107,10 +115,9 @@ wgrad_reduce_all_kernel(const WgradReduceDesc* __restrict__ descs, float* __rest
   if (d.stem) {
     const int total = 256 * d.cout;
     for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < total; i += gridDim.x * blockDim.x) {
-      const int co = i >> 8, k = i & 255;
-      const int rp = k >> 6, sp_ = (k >> 4) & 3, ph = (k >> 3) & 1, pw = (k >> 2) & 1, c = k & 3;
-      const int r = 2 * rp + ph - 1, s = 2 * sp_ + pw - 1;
-      if (c >= 3 || r < 0 || s < 0) continue;
+      const int co = i >> 8;
+      int c, r, s;
+      if (!stem_tap(i & 255, c, r, s)) continue;
       float acc = 0.f;
       for (int sp = 0; sp < d.splits; ++sp) acc += d.partial[(int64_t)sp * total + i];
       dw[((co * 3 + c) * 7 + r) * 7 + s] += acc;
@@ -151,11 +158,10 @@ __global__ void prep_weights_all_kernel(const float* __restrict__ params, const 
   if (d.stem) {
     const int total = d.cout * 256;
     for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < total; i += gridDim.x * blockDim.x) {
-      const int co = i >> 8, k = i & 255;
-      const int rp = k >> 6, sp = (k >> 4) & 3, ph = (k >> 3) & 1, pw = (k >> 2) & 1, c = k & 3;
-      const int r = 2 * rp + ph - 1, s = 2 * sp + pw - 1;
+      const int co = i >> 8;
+      int c, r, s;
       float v = 0.f;
-      if (c < 3 && r >= 0 && s >= 0 && r < 7 && s < 7) v = w[((co * 3 + c) * 7 + r) * 7 + s];
+      if (stem_tap(i & 255, c, r, s)) v = w[((co * 3 + c) * 7 + r) * 7 + s];
       d.wf[i] = __float2bfloat16_rn(v);
     }
     return;
@@ -304,8 +310,9 @@ int dirb200_conv_dgrad(const void* dy, const void* w_dgrad, void* dx, int n, int
 size_t dirb200_conv_wgrad_workspace_bytes(int n, int h, int w, int cin, int cout, int kh, int kw, int stride, int pad,
                                           int stem) {
   ConvShape s;
-  if (to_shape(n, h, w, cin, cout, kh, kw, stride, pad, stem, &s)) return 0;
-  return conv_wgrad_workspace_bytes(s);
+  ConvPlan pl;
+  if (to_shape(n, h, w, cin, cout, kh, kw, stride, pad, stem, &s) || plan_conv(s, stem != 0, 2, &pl)) return 0;
+  return pl.workspace_bytes;
 }
 
 int dirb200_conv_wgrad(const void* x, const void* dy, float* dw, void* workspace, size_t workspace_bytes, int n, int h,
@@ -314,8 +321,10 @@ int dirb200_conv_wgrad(const void* x, const void* dy, float* dw, void* workspace
   DIRB_CHECK_ARG(x && dy && dw && workspace, "conv_wgrad: null pointer");
   ConvShape s;
   if (int rc = to_shape(n, h, w, cin, cout, kh, kw, stride, pad, stem, &s)) return rc;
-  if (workspace_bytes < conv_wgrad_workspace_bytes(s)) {
-    set_error("conv_wgrad: workspace too small (%zu < %zu)", workspace_bytes, conv_wgrad_workspace_bytes(s));
+  ConvPlan pl;
+  if (int rc = plan_conv(s, stem != 0, 2, &pl)) return rc;
+  if (workspace_bytes < pl.workspace_bytes) {
+    set_error("conv_wgrad: workspace too small (%zu < %zu)", workspace_bytes, pl.workspace_bytes);
     return DIRB200_ERR_WORKSPACE;
   }
   return conv_wgrad((const __nv_bfloat16*)x, (const __nv_bfloat16*)dy, dw, (float*)workspace, s, stem != 0,
@@ -367,8 +376,8 @@ int dirb200_conv_dgrad_bn_moments(const void* dy, const void* w_dgrad, void* dx,
   return DIRB200_OK;
 }
 
-/* Host-only (no CUDA call): the GEMM form dirb200_conv_fprop / _dgrad / _wgrad (op 0 / 1 / 2) would launch for this
- * shape: plan7[0] tile width BN, [1] 0 (no CTA pairs), [2] A-operand form (0 cp.async gather, 1 tiled TMA, 2 im2col
+/* Host-only (no CUDA call): the plan dirb200_conv_fprop / _dgrad / _wgrad (op 0 / 1 / 2) would execute for this
+ * shape, or the status they would refuse it with: plan7[0] tile width BN, [1] 0 (no CTA pairs), [2] A-operand form (0 cp.async gather, 1 tiled TMA, 2 im2col
  * TMA), [3] 0 (no patch-resident form), [4] split-K factor, [5] launches, [6] dgrad can carry the BN-backward moments of
  * the previous layer. */
 int dirb200_conv_plan(int n, int h, int w, int cin, int cout, int kh, int kw, int stride, int pad, int stem, int op,
@@ -376,7 +385,11 @@ int dirb200_conv_plan(int n, int h, int w, int cin, int cout, int kh, int kw, in
   DIRB_CHECK_ARG(plan7 && op >= 0 && op <= 2, "conv_plan: bad arguments");
   ConvShape s;
   if (int rc = to_shape(n, h, w, cin, cout, kh, kw, stride, pad, stem, &s)) return rc;
-  return conv_plan(s, stem != 0, op, plan7);
+  ConvPlan pl;
+  if (int rc = plan_conv(s, stem != 0, op, &pl)) return rc;
+  const int v[7] = {pl.bn, 0, pl.a_form, 0, pl.splits, pl.nlaunch, pl.fuses_bn_moments ? 1 : 0};
+  for (int i = 0; i < 7; ++i) plan7[i] = v[i];
+  return DIRB200_OK;
 }
 
 int dirb200_prep_weights_all(const float* params, const dirb200_prep_job* jobs_host, int njobs, void* stream) {

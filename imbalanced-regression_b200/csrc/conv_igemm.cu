@@ -22,7 +22,6 @@ constexpr int BM = 128;  // GEMM rows per tile (pixels; for wgrad: 2 chunks x 64
 constexpr int BK = 64;   // bf16 elements per k-block = one 128-byte swizzle row
 constexpr int kProducerThreads = 128;   // warpgroup 0
 constexpr int kThreads = 384;           // + two consumer warpgroups
-constexpr int kMaxTaps = 25;   // up to 5x5 filters (the NYUD2 decoder / refinement convs, nyud2-dir/models/modules.py:11-20,154-160)
 constexpr int kMaxSmemBytes = 232448;   // opt-in shared memory per block (227 KB)
 
 struct IgemmParams {
@@ -723,7 +722,6 @@ int make_tmap_im2col_bf16(CUtensorMap* tm, const void* ptr, int c, int w, int h,
     reinterpret_cast<uint64_t*>(tm)[1] &= ~(1ull << 21);
   return DIRB200_OK;
 }
-static thread_local StatLayout t_last_layout{};     // row layout of the statistics the most recent fprop launch wrote
 
 // Host-side completion of the launch parameters: reciprocal constants for every run-time divisor the kernel meets and
 // the per-tap tables (gather offset, im2col offsets) indexed by the position in tap_list.
@@ -765,7 +763,8 @@ static IgemmParams finish_params(const IgemmParams& P) {
 }
 
 template <int BN, bool WGRAD, bool STEM, bool ATMA = false, bool AFFINE = false, bool BSTAT = false>
-static int launch_igemm_impl(const CUtensorMap& tm, const CUtensorMap& tma, const IgemmParams& Qin, cudaStream_t st) {
+static int launch_igemm_impl(const CUtensorMap& tm, const CUtensorMap& tma, const IgemmParams& Qin, int grid,
+                             cudaStream_t st) {
   using C = Cfg<BN, !WGRAD>;
   const IgemmParams Q = finish_params(Qin);
   static bool configured = false;
@@ -774,11 +773,6 @@ static int launch_igemm_impl(const CUtensorMap& tm, const CUtensorMap& tma, cons
                                    cudaFuncAttributeMaxDynamicSharedMemorySize, C::kSmemBytes));
     configured = true;
   }
-  int grid = Q.num_tiles < num_sms() ? Q.num_tiles : num_sms();
-  // fprop / dgrad CTAs each keep one n_tile: at least one CTA per n_tile, also when DIRB200_SMS caps the SM count
-  // below the tile count (the extra CTAs run as a second wave)
-  if (!WGRAD && grid < Q.n_tiles) grid = Q.n_tiles;
-  t_last_layout = StatLayout{grid, Q.n_tiles, BN, 1};
   igemm_kernel<BN, WGRAD, STEM, ATMA, AFFINE, BSTAT><<<grid, kThreads, C::kSmemBytes, st>>>(tm, tma, Q);
   DIRB_LAUNCHED();
   return DIRB200_OK;
@@ -786,29 +780,26 @@ static int launch_igemm_impl(const CUtensorMap& tm, const CUtensorMap& tma, cons
 
 // tma != nullptr: the A operand is loaded by TMA too (tiled or im2col map, P.a_mode)
 template <int BN, bool WGRAD, bool STEM>
-static int launch_igemm(const CUtensorMap& tm, const IgemmParams& P, int m_tiles, int splits, cudaStream_t st,
+static int launch_igemm(const CUtensorMap& tm, const IgemmParams& Q, int grid, cudaStream_t st,
                         const CUtensorMap* tma = nullptr) {
-  IgemmParams Q = P;
-  Q.m_tiles = m_tiles;
-  Q.num_tiles = m_tiles * P.n_tiles * splits;
   if constexpr (!STEM) {
     if (tma) {
       if constexpr (!WGRAD) {
-        if (Q.epi_scale != nullptr) return launch_igemm_impl<BN, false, false, true, true>(tm, *tma, Q, st);
-        if (Q.bst_y != nullptr) return launch_igemm_impl<BN, false, false, true, false, true>(tm, *tma, Q, st);
+        if (Q.epi_scale != nullptr) return launch_igemm_impl<BN, false, false, true, true>(tm, *tma, Q, grid, st);
+        if (Q.bst_y != nullptr) return launch_igemm_impl<BN, false, false, true, false, true>(tm, *tma, Q, grid, st);
       }
-      return launch_igemm_impl<BN, WGRAD, false, true>(tm, *tma, Q, st);
+      return launch_igemm_impl<BN, WGRAD, false, true>(tm, *tma, Q, grid, st);
     }
   }
   if constexpr (!WGRAD && !STEM) {
     // gather-fed fprop (DIRB200_ATMA=0 / DIRB200_IM2COL=0): the folded-BN epilogue works the same way
-    if (Q.epi_scale != nullptr) return launch_igemm_impl<BN, false, false, false, true>(tm, tm, Q, st);
+    if (Q.epi_scale != nullptr) return launch_igemm_impl<BN, false, false, false, true>(tm, tm, Q, grid, st);
   }
   if (Q.epi_scale != nullptr || Q.bst_y != nullptr) {
     set_error("conv: the BN-backward moments epilogue needs a TMA-fed A operand; the folded-BN one a non-stem fprop");
     return DIRB200_ERR_ARG;
   }
-  return launch_igemm_impl<BN, WGRAD, STEM>(tm, tm, Q, st);
+  return launch_igemm_impl<BN, WGRAD, STEM>(tm, tm, Q, grid, st);
 }
 
 // GEMM-N tile width: 128 where N allows (a consumer warpgroup's 64 x 128 fp32 accumulators take 64 registers per
@@ -840,12 +831,7 @@ static bool atma_enabled() {
   }();
   return on;
 }
-static bool is_plain_gemm(const ConvShape& s, bool stem) {
-  return !stem && s.kh == 1 && s.kw == 1 && s.stride == 1 && s.pad == 0 && atma_enabled();
-}
-// Every other non-stem conv (3x3, strided) takes its A operand through im2col-mode TMA (fprop, stride-1 dgrad, wgrad);
-// (incl. the parity classes of a stride-2 dgrad); only the stem keeps the cp.async gather.  DIRB200_IM2COL=0: gather
-// for all of those.
+// DIRB200_IM2COL=0: the cp.async gather for the convs that would take im2col-mode TMA.
 static bool im2col_enabled() {
   static const bool on = [] {
     const char* e = getenv("DIRB200_IM2COL");
@@ -854,176 +840,10 @@ static bool im2col_enabled() {
   return on && atma_enabled();
 }
 
-// Y[n,ho,wo,cout] = conv(X[n,h,w,cin], W[cout][kh][kw][cin])
-static int conv_fprop_impl(const __nv_bfloat16* x, const __nv_bfloat16* w, __nv_bfloat16* y, const ConvShape& s, bool stem,
-                           cudaStream_t st, float* stat_partial, const ConvEpilogue* epi);
-
-int conv_fprop(const __nv_bfloat16* x, const __nv_bfloat16* w, __nv_bfloat16* y, const ConvShape& s, bool stem,
-               cudaStream_t st, float* stat_partial, StatLayout* layout) {
-  const int rc = conv_fprop_impl(x, w, y, s, stem, st, stat_partial, nullptr);
-  if (layout) *layout = t_last_layout;
-  return rc;
-}
-
-int conv_fprop_affine(const __nv_bfloat16* x, const __nv_bfloat16* w, __nv_bfloat16* out, const ConvShape& s,
-                      const ConvEpilogue& epi, cudaStream_t st) {
-  DIRB_CHECK_ARG(epi.scale && epi.shift, "conv_fprop_affine: scale / shift missing");
-  return conv_fprop_impl(x, w, out, s, false, st, nullptr, &epi);
-}
-
-static int conv_fprop_impl(const __nv_bfloat16* x, const __nv_bfloat16* w, __nv_bfloat16* y, const ConvShape& s, bool stem,
-                           cudaStream_t st, float* stat_partial, const ConvEpilogue* epi) {
-  if (int rc = check_shape(s, stem, "conv_fprop")) return rc;
-  const int ktot = s.kh * s.kw * s.cin;
-  IgemmParams P{};
-  P.src = x; P.n = s.n; P.hs = s.h; P.ws = s.w; P.cs = s.cin; P.hm = s.ho; P.wm = s.wo;
-  P.kh = s.kh; P.kw = s.kw; P.stride = s.stride; P.pad = s.pad; P.transposed = 0;
-  P.cpb = stem ? 1 : s.cin / 64;
-  P.pixels = static_cast<long long>(s.n) * s.ho * s.wo;
-  P.num_kblocks = ktot / 64;
-  P.ntaps_c = s.kh * s.kw;
-  DIRB_CHECK_ARG(stem || P.ntaps_c <= kMaxTaps, "conv_fprop: at most %d filter taps (got %dx%d)", kMaxTaps, s.kh, s.kw);
-  for (int i = 0; i < kMaxTaps; ++i) P.tap_list[i] = i;
-  P.ldc = s.cout; P.out = y;
-  P.stat_out = stat_partial;
-  if (epi) {
-    P.epi_scale = epi->scale; P.epi_shift = epi->shift; P.epi_res = epi->residual; P.epi_relu = epi->relu ? 1 : 0;
-  }
-  const int m_tiles = static_cast<int>((P.pixels + BM - 1) / BM);
-  const int bn = pick_bn(s.cout);
-  P.n_tiles = s.cout / bn;
-  CUtensorMap tm, ta;
-  bool tma_fed = false;
-  if (is_plain_gemm(s, stem)) {         // x as [pixels][cin]
-    if (int rc = make_tmap_bf16_2d(&ta, x, s.cin, static_cast<uint64_t>(P.pixels), static_cast<uint64_t>(s.cin) * 2, BM))
-      return rc;
-    P.a_mode = 1;
-    tma_fed = true;
-  } else if (!stem && im2col_enabled()) {   // x [n,h,w,cin], base pixel (ho*stride - pad, wo*stride - pad)
-    if (int rc = make_tmap_im2col_bf16(&ta, x, s.cin, s.w, s.h, s.n, -s.pad, -s.pad, s.pad - (s.kw - 1),
-                                       s.pad - (s.kh - 1), s.stride, BM))
-      return rc;
-    P.a_mode = 2; P.i2c_stride = s.stride; P.i2c_lo = -s.pad;
-    tma_fed = true;
-  }
-  if (int rc = make_tmap_bf16_2d(&tm, w, ktot, s.cout, static_cast<uint64_t>(ktot) * 2, bn)) return rc;
-  if (stem) return DISPATCH_BN(bn, false, true, tm, P, m_tiles, 1, st);
-  if (tma_fed) return DISPATCH_BN(bn, false, false, tm, P, m_tiles, 1, st, &ta);
-  return DISPATCH_BN(bn, false, false, tm, P, m_tiles, 1, st);
-}
-
-// dX[n,h,w,cin] = conv_transpose(dY[n,ho,wo,cout], Wt[cin][kh][kw][cout])
-bool conv_dgrad_fuses_bn_moments(const ConvShape& s) {
-  return s.stride == 1 && (is_plain_gemm(s, false) || (im2col_enabled() && s.kh == s.kw));
-}
-
-int conv_dgrad(const __nv_bfloat16* dy, const __nv_bfloat16* wt, __nv_bfloat16* dx, const ConvShape& s,
-               cudaStream_t st, const DgradBnMoments* bnm) {
-  if (int rc = check_shape(s, false, "conv_dgrad")) return rc;
-  DIRB_CHECK_ARG(!bnm || (conv_dgrad_fuses_bn_moments(s) && bnm->y && bnm->scale && bnm->shift && bnm->partial),
-                 "conv_dgrad: BN-backward moments are fused into TMA-fed stride-1 dgrads only");
-  DIRB_CHECK_ARG(s.stride == 1 || s.stride == 2, "conv_dgrad: stride must be 1 or 2 (got %d)", s.stride);
-  DIRB_CHECK_ARG(s.kh * s.kw <= (s.stride == 1 ? kMaxTaps : 9), "conv_dgrad: at most %d filter taps (stride 2: 9; got %dx%d)",
-                 kMaxTaps, s.kh, s.kw);
-  const int ktot = s.kh * s.kw * s.cout;
-  IgemmParams P{};
-  P.src = dy; P.n = s.n; P.hs = s.ho; P.ws = s.wo; P.cs = s.cout; P.hm = s.h; P.wm = s.w;
-  P.kh = s.kh; P.kw = s.kw; P.stride = s.stride; P.pad = s.pad; P.transposed = 1;
-  P.cpb = s.cout / 64;
-  P.ldc = s.cin; P.out = dx;
-  if (bnm) {
-    P.bst_y = bnm->y; P.bst_scale = bnm->scale; P.bst_shift = bnm->shift; P.stat_out = bnm->partial;
-  }
-  const int bn = pick_bn(s.cin);
-  CUtensorMap tm;
-  if (int rc = make_tmap_bf16_2d(&tm, wt, ktot, s.cin, static_cast<uint64_t>(ktot) * 2, bn)) return rc;
-  if (s.stride == 1) {
-    P.pixels = static_cast<long long>(s.n) * s.h * s.w;
-    P.ntaps_c = s.kh * s.kw;
-    for (int i = 0; i < kMaxTaps; ++i) P.tap_list[i] = i;
-    P.num_kblocks = ktot / 64;
-    const int m_tiles = static_cast<int>((P.pixels + BM - 1) / BM);
-    P.n_tiles = s.cin / bn;
-    CUtensorMap ta;
-    bool tma_fed = false;
-    if (is_plain_gemm(s, false)) {      // dy as [pixels][cout]
-      if (int rc = make_tmap_bf16_2d(&ta, dy, s.cout, static_cast<uint64_t>(P.pixels), static_cast<uint64_t>(s.cout) * 2, BM))
-        return rc;
-      P.a_mode = 1;
-      tma_fed = true;
-    } else if (im2col_enabled() && s.kh == s.kw) {
-      // dy [n,ho,wo,cout], base pixel (y + pad - (k-1), x + pad - (k-1)), tap offsets reversed
-      const int lo = s.pad - (s.kh - 1);
-      if (int rc = make_tmap_im2col_bf16(&ta, dy, s.cout, s.wo, s.ho, s.n, lo, lo, lo + s.w - s.wo, lo + s.h - s.ho, 1, BM))
-        return rc;
-      P.a_mode = 2; P.i2c_stride = 1; P.i2c_lo = lo;
-      tma_fed = true;
-    }
-    const int rc = tma_fed ? DISPATCH_BN(bn, false, false, tm, P, m_tiles, 1, st, &ta)
-                           : DISPATCH_BN(bn, false, false, tm, P, m_tiles, 1, st);
-    if (bnm && bnm->layout) *bnm->layout = t_last_layout;
-    return rc;
-  }
-  // stride 2: one launch per output-pixel parity class; a class without any tap receives no gradient (zeros)
-  bool need_zero = false;
-  for (int cls = 0; cls < 4; ++cls) {
-    const int py = cls >> 1, px = cls & 1;
-    int nt = 0;
-    for (int r = 0; r < s.kh; ++r)
-      for (int q = 0; q < s.kw; ++q)
-        if (((py + s.pad - r) & 1) == 0 && ((px + s.pad - q) & 1) == 0) ++nt;
-    if (nt == 0) need_zero = true;
-  }
-  if (need_zero)
-    DIRB_CUDA(cudaMemsetAsync(dx, 0, static_cast<size_t>(s.n) * s.h * s.w * s.cin * sizeof(__nv_bfloat16), st));
-  for (int cls = 0; cls < 4; ++cls) {
-    IgemmParams Q = P;
-    Q.cls_on = 1; Q.cls_py = cls >> 1; Q.cls_px = cls & 1; Q.full_h = s.h; Q.full_w = s.w;
-    Q.hm = (s.h - Q.cls_py + 1) / 2;
-    Q.wm = (s.w - Q.cls_px + 1) / 2;
-    Q.ntaps_c = 0;
-    for (int r = 0; r < s.kh; ++r)
-      for (int q = 0; q < s.kw; ++q)
-        if (((Q.cls_py + s.pad - r) & 1) == 0 && ((Q.cls_px + s.pad - q) & 1) == 0) Q.tap_list[Q.ntaps_c++] = r * s.kw + q;
-    if (Q.ntaps_c == 0 || Q.hm <= 0 || Q.wm <= 0) continue;
-    Q.pixels = static_cast<long long>(s.n) * Q.hm * Q.wm;
-    Q.num_kblocks = Q.ntaps_c * Q.cpb;
-    const int m_tiles = static_cast<int>((Q.pixels + BM - 1) / BM);
-    Q.n_tiles = s.cin / bn;
-    if (im2col_enabled()) {
-      // the class is a stride-1 "convolution" over the dy grid whose taps sit at offsets (py + pad - r) / 2: im2col-mode
-      // TMA with the base-pixel box [lo, lo + class grid) (out-of-range dy pixels arrive as zeros)
-      int lo = 1 << 20;
-      for (int i = 0; i < Q.ntaps_c; ++i) {
-        const int r = Q.tap_list[i] / s.kw, q = Q.tap_list[i] % s.kw;
-        const int orr = (Q.cls_py + s.pad - r) / 2, oq = (Q.cls_px + s.pad - q) / 2;
-        lo = orr < lo ? orr : lo;
-        lo = oq < lo ? oq : lo;
-      }
-      CUtensorMap ta;
-      if (int rc = make_tmap_im2col_bf16(&ta, dy, s.cout, s.wo, s.ho, s.n, lo, lo, lo + Q.wm - s.wo, lo + Q.hm - s.ho, 1, BM))
-        return rc;
-      Q.a_mode = 2; Q.i2c_stride = 1; Q.i2c_lo = lo;
-      if (int rc = DISPATCH_BN(bn, false, false, tm, Q, m_tiles, 1, st, &ta)) return rc;
-      continue;
-    }
-    if (int rc = DISPATCH_BN(bn, false, false, tm, Q, m_tiles, 1, st)) return rc;
-  }
-  return DIRB200_OK;
-}
-
-static int wgrad_bn(const ConvShape& s) { return pick_bn(s.cout); }
-
 // Split-K factor of the wgrad GEMM (K = pixels).  The persistent CTAs walk tiles x splits work items in waves of
 // num_sms; one item costs its k-blocks plus an epilogue worth ~6 k-blocks (128 x BN fp32 partials; an estimate, not
 // re-measured on H100), so a launch costs about waves x (k-blocks per split + 6); the minimiser avoids straggler waves.
-int conv_wgrad_splits(const ConvShape& s) {
-  const long long pixels = static_cast<long long>(s.n) * s.ho * s.wo;
-  const int kblocks = static_cast<int>((pixels + 63) / 64);
-  const int chunks = s.kh * s.kw * s.cin / 64;
-  const int bn = wgrad_bn(s);
-  const int m_tiles = (chunks + 1) / 2;
-  const int tiles = m_tiles * (s.cout / bn);
+static int wgrad_splits(int kblocks, int tiles) {
   const int sms = num_sms();
   int max_splits = (kblocks + 7) / 8;                   // at least 8 k-blocks per split
   if (max_splits < 1) max_splits = 1;
@@ -1043,92 +863,220 @@ int conv_wgrad_splits(const ConvShape& s) {
   return best;
 }
 
-size_t conv_wgrad_workspace_bytes(const ConvShape& s) {
-  return static_cast<size_t>(conv_wgrad_splits(s)) * s.kh * s.kw * s.cin * s.cout * sizeof(float);
+int plan_conv(const ConvShape& s, bool stem, int op, ConvPlan* pl) {
+  static const char* const kWho[3] = {"conv_fprop", "conv_dgrad", "conv_wgrad"};
+  *pl = ConvPlan{};
+  if (int rc = check_shape(s, stem, kWho[op])) return rc;
+  const bool dgrad = op == 1, wgrad = op == 2;
+  const int taps = s.kh * s.kw;
+  DIRB_CHECK_ARG(!(dgrad && stem), "conv_dgrad: the stem has no data gradient");
+  DIRB_CHECK_ARG(!dgrad || s.stride == 1 || s.stride == 2, "conv_dgrad: stride must be 1 or 2 (got %d)", s.stride);
+  const int max_taps = dgrad && s.stride == 2 ? 9 : kMaxTaps;
+  DIRB_CHECK_ARG(stem || taps <= max_taps, "%s: at most %d filter taps (got %dx%d)", kWho[op], max_taps, s.kh, s.kw);
+
+  pl->op = op;
+  pl->stem = stem;
+  const int n_dim = dgrad ? s.cin : s.cout;
+  const int cs = dgrad ? s.cout : s.cin;        // channels of the gathered tensor (dgrad: dy)
+  pl->bn = pick_bn(n_dim);
+  pl->n_tiles = n_dim / pl->bn;
+  // A operand: 1x1 stride-1 GEMMs read a plain [pixels][channels] matrix by tiled TMA; every other non-stem conv takes
+  // im2col-mode TMA, except a stride-1 dgrad with a non-square filter (one box offset serves both axes there); the stem
+  // keeps the cp.async gather
+  const bool plain = !stem && s.kh == 1 && s.kw == 1 && s.stride == 1 && s.pad == 0 && atma_enabled();
+  pl->a_form = plain ? 1 : (!stem && im2col_enabled() && !(dgrad && s.stride == 1 && s.kh != s.kw)) ? 2 : 0;
+  pl->fuses_bn_moments = dgrad && s.stride == 1 && pl->a_form != 0;
+  pl->classes = dgrad && s.stride == 2;
+  pl->splits = 1;
+
+  for (int cls = 0; cls < (pl->classes ? 4 : 1); ++cls) {
+    ConvLaunch L{};
+    if (pl->classes) {
+      // output pixels (2y' + py, 2x' + px) receive only the taps whose parity matches: quarter-size grids
+      L.cls_py = cls >> 1;
+      L.cls_px = cls & 1;
+      L.hm = (s.h - L.cls_py + 1) / 2;
+      L.wm = (s.w - L.cls_px + 1) / 2;
+      for (int r = 0; r < s.kh; ++r)
+        for (int q = 0; q < s.kw; ++q)
+          if (((L.cls_py + s.pad - r) & 1) == 0 && ((L.cls_px + s.pad - q) & 1) == 0) L.taps[L.ntaps++] = r * s.kw + q;
+      if (L.ntaps == 0) pl->need_zero = true;
+      if (L.ntaps == 0 || L.hm <= 0 || L.wm <= 0) continue;
+      L.num_kblocks = L.ntaps * (cs / 64);
+    } else {
+      L.hm = dgrad ? s.h : s.ho;
+      L.wm = dgrad ? s.w : s.wo;
+      L.ntaps = taps;
+      for (int i = 0; i < kMaxTaps; ++i) L.taps[i] = i;
+      L.num_kblocks = taps * cs / 64;
+    }
+    L.pixels = static_cast<long long>(s.n) * L.hm * L.wm;
+    if (wgrad) {
+      L.num_kblocks = static_cast<int>((L.pixels + 63) / 64);
+      L.m_tiles = (taps * cs / 64 + 1) / 2;         // pairs of 64-row chunks of the K_total x Cout result
+      pl->splits = wgrad_splits(L.num_kblocks, L.m_tiles * pl->n_tiles);
+      pl->kblocks_per_split = (L.num_kblocks + pl->splits - 1) / pl->splits;
+      pl->workspace_bytes = static_cast<size_t>(pl->splits) * taps * s.cin * s.cout * sizeof(float);
+    } else {
+      L.m_tiles = static_cast<int>((L.pixels + BM - 1) / BM);
+    }
+    if (pl->a_form == 2 && !dgrad) {              // x [n,h,w,cin], base pixel (ho*stride - pad, wo*stride - pad)
+      L.i2c_stride = s.stride;
+      L.i2c_lo = L.i2c_lower_w = L.i2c_lower_h = -s.pad;
+      L.i2c_upper_w = s.pad - (s.kw - 1);
+      L.i2c_upper_h = s.pad - (s.kh - 1);
+    } else if (pl->a_form == 2) {
+      // dy [n,ho,wo,cout]: a stride-1 "convolution" over the dy grid whose taps sit at offsets pad - r (tap offsets
+      // reversed) or, for a parity class, (py + pad - r) / 2; the base-pixel box is [lo, lo + row grid) with lo the
+      // lowest offset (out-of-range dy pixels arrive as zeros)
+      int lo = s.pad - (s.kh - 1);
+      if (pl->classes) {
+        lo = 1 << 20;
+        for (int i = 0; i < L.ntaps; ++i) {
+          const int r = L.taps[i] / s.kw, q = L.taps[i] % s.kw;
+          const int orr = (L.cls_py + s.pad - r) / 2, oq = (L.cls_px + s.pad - q) / 2;
+          lo = orr < lo ? orr : lo;
+          lo = oq < lo ? oq : lo;
+        }
+      }
+      L.i2c_stride = 1;
+      L.i2c_lo = L.i2c_lower_w = L.i2c_lower_h = lo;
+      L.i2c_upper_w = lo + L.wm - s.wo;
+      L.i2c_upper_h = lo + L.hm - s.ho;
+    }
+    const int tiles = L.m_tiles * pl->n_tiles * pl->splits;
+    L.grid = tiles < num_sms() ? tiles : num_sms();
+    // fprop / dgrad CTAs each keep one n_tile: at least one CTA per n_tile, also when DIRB200_SMS caps the SM count
+    // below the tile count (the extra CTAs run as a second wave)
+    if (!wgrad && L.grid < pl->n_tiles) L.grid = pl->n_tiles;
+    pl->launch[pl->nlaunch++] = L;
+  }
+  if (!wgrad && !pl->classes) pl->layout = StatLayout{pl->launch[0].grid, pl->n_tiles, pl->bn, 1};
+  return DIRB200_OK;
+}
+
+// Runs every launch of a plan.  P0 holds the tensor pointers (src: the gathered tensor, out) and the epilogue
+// options; b is the B operand (fprop / dgrad: the weights [N][K], K-major; wgrad: dy [pixels][cout]).
+static int run_plan(const ConvShape& s, const ConvPlan& pl, const IgemmParams& P0, const void* b, cudaStream_t st) {
+  const bool dgrad = pl.op == 1, wgrad = pl.op == 2;
+  CUtensorMap tm;
+  if (wgrad) {
+    if (int rc = make_tmap_bf16_2d(&tm, b, s.cout, static_cast<uint64_t>(pl.launch[0].pixels),
+                                   static_cast<uint64_t>(s.cout) * 2, 64))
+      return rc;
+  } else {
+    const int ktot = s.kh * s.kw * (dgrad ? s.cout : s.cin);
+    if (int rc = make_tmap_bf16_2d(&tm, b, ktot, dgrad ? s.cin : s.cout, static_cast<uint64_t>(ktot) * 2, pl.bn))
+      return rc;
+  }
+  if (pl.need_zero)
+    DIRB_CUDA(cudaMemsetAsync(P0.out, 0, static_cast<size_t>(s.n) * s.h * s.w * s.cin * sizeof(__nv_bfloat16), st));
+  for (int i = 0; i < pl.nlaunch; ++i) {
+    const ConvLaunch& L = pl.launch[i];
+    IgemmParams P = P0;
+    P.n = s.n;
+    P.hs = dgrad ? s.ho : s.h;
+    P.ws = dgrad ? s.wo : s.w;
+    P.cs = dgrad ? s.cout : s.cin;
+    P.hm = L.hm;
+    P.wm = L.wm;
+    P.kh = s.kh; P.kw = s.kw; P.stride = s.stride; P.pad = s.pad; P.transposed = dgrad ? 1 : 0;
+    if (pl.classes) {
+      P.cls_on = 1; P.cls_py = L.cls_py; P.cls_px = L.cls_px; P.full_h = s.h; P.full_w = s.w;
+    }
+    P.ntaps_c = L.ntaps;
+    for (int t = 0; t < kMaxTaps; ++t) P.tap_list[t] = L.taps[t];
+    P.cpb = pl.stem ? 1 : P.cs / 64;
+    P.pixels = L.pixels;
+    P.num_kblocks = L.num_kblocks;
+    P.kblocks_per_split = pl.kblocks_per_split;
+    if (wgrad) P.total_chunks = s.kh * s.kw * s.cin / 64;
+    P.m_tiles = L.m_tiles;
+    P.n_tiles = pl.n_tiles;
+    P.num_tiles = L.m_tiles * pl.n_tiles * pl.splits;
+    P.a_mode = pl.a_form;
+    P.i2c_stride = L.i2c_stride;
+    P.i2c_lo = L.i2c_lo;
+    P.ldc = dgrad ? s.cin : s.cout;
+    // the A operand's map: the gathered tensor as a plain [pixels][channels] matrix, or in im2col mode; boxes of
+    // 64 channels x one tile's rows (wgrad: one 64-pixel k-block)
+    const uint32_t rows = wgrad ? 64 : BM;
+    CUtensorMap ta;
+    if (pl.a_form == 1) {
+      if (int rc = make_tmap_bf16_2d(&ta, P.src, P.cs, static_cast<uint64_t>(P.pixels), static_cast<uint64_t>(P.cs) * 2,
+                                     rows))
+        return rc;
+    } else if (pl.a_form == 2) {
+      if (int rc = make_tmap_im2col_bf16(&ta, P.src, P.cs, P.ws, P.hs, P.n, L.i2c_lower_w, L.i2c_lower_h, L.i2c_upper_w,
+                                         L.i2c_upper_h, L.i2c_stride, rows))
+        return rc;
+    }
+    const CUtensorMap* pa = pl.a_form != 0 ? &ta : nullptr;
+    int rc;
+    if (pl.stem)
+      rc = wgrad ? DISPATCH_BN(pl.bn, true, true, tm, P, L.grid, st) : DISPATCH_BN(pl.bn, false, true, tm, P, L.grid, st);
+    else
+      rc = wgrad ? DISPATCH_BN(pl.bn, true, false, tm, P, L.grid, st, pa)
+                 : DISPATCH_BN(pl.bn, false, false, tm, P, L.grid, st, pa);
+    if (rc) return rc;
+  }
+  return DIRB200_OK;
+}
+
+// Y[n,ho,wo,cout] = conv(X[n,h,w,cin], W[cout][kh][kw][cin])
+static int conv_fprop_impl(const __nv_bfloat16* x, const __nv_bfloat16* w, __nv_bfloat16* y, const ConvShape& s, bool stem,
+                           cudaStream_t st, float* stat_partial, const ConvEpilogue* epi, StatLayout* layout) {
+  ConvPlan pl;
+  if (int rc = plan_conv(s, stem, 0, &pl)) return rc;
+  IgemmParams P{};
+  P.src = x; P.out = y;
+  P.stat_out = stat_partial;
+  if (epi) {
+    P.epi_scale = epi->scale; P.epi_shift = epi->shift; P.epi_res = epi->residual; P.epi_relu = epi->relu ? 1 : 0;
+  }
+  if (int rc = run_plan(s, pl, P, w, st)) return rc;
+  if (layout) *layout = pl.layout;
+  return DIRB200_OK;
+}
+
+int conv_fprop(const __nv_bfloat16* x, const __nv_bfloat16* w, __nv_bfloat16* y, const ConvShape& s, bool stem,
+               cudaStream_t st, float* stat_partial, StatLayout* layout) {
+  return conv_fprop_impl(x, w, y, s, stem, st, stat_partial, nullptr, layout);
+}
+
+int conv_fprop_affine(const __nv_bfloat16* x, const __nv_bfloat16* w, __nv_bfloat16* out, const ConvShape& s,
+                      const ConvEpilogue& epi, cudaStream_t st) {
+  DIRB_CHECK_ARG(epi.scale && epi.shift, "conv_fprop_affine: scale / shift missing");
+  return conv_fprop_impl(x, w, out, s, false, st, nullptr, &epi, nullptr);
+}
+
+// dX[n,h,w,cin] = conv_transpose(dY[n,ho,wo,cout], Wt[cin][kh][kw][cout]); stride 2: one launch per output-pixel
+// parity class, a class without any tap receives no gradient (zeros)
+int conv_dgrad(const __nv_bfloat16* dy, const __nv_bfloat16* wt, __nv_bfloat16* dx, const ConvShape& s,
+               cudaStream_t st, const DgradBnMoments* bnm) {
+  ConvPlan pl;
+  if (int rc = plan_conv(s, false, 1, &pl)) return rc;
+  DIRB_CHECK_ARG(!bnm || (pl.fuses_bn_moments && bnm->y && bnm->scale && bnm->shift && bnm->partial),
+                 "conv_dgrad: BN-backward moments are fused into TMA-fed stride-1 dgrads only");
+  IgemmParams P{};
+  P.src = dy; P.out = dx;
+  if (bnm) {
+    P.bst_y = bnm->y; P.bst_scale = bnm->scale; P.bst_shift = bnm->shift; P.stat_out = bnm->partial;
+  }
+  if (int rc = run_plan(s, pl, P, wt, st)) return rc;
+  if (bnm && bnm->layout) *bnm->layout = pl.layout;
+  return DIRB200_OK;
 }
 
 // partial[split][cout][(r,s,c)] = sum over the split's pixels of X_gathered^T dY
 int conv_wgrad_partials(const __nv_bfloat16* x, const __nv_bfloat16* dy, float* partial, const ConvShape& s, bool stem,
                         int* splits_out, cudaStream_t st) {
-  if (int rc = check_shape(s, stem, "conv_wgrad")) return rc;
+  ConvPlan pl;
+  if (int rc = plan_conv(s, stem, 2, &pl)) return rc;
   IgemmParams P{};
-  P.src = x; P.n = s.n; P.hs = s.h; P.ws = s.w; P.cs = s.cin; P.hm = s.ho; P.wm = s.wo;
-  P.kh = s.kh; P.kw = s.kw; P.stride = s.stride; P.pad = s.pad; P.transposed = 0;
-  P.cpb = stem ? 1 : s.cin / 64;
-  P.pixels = static_cast<long long>(s.n) * s.ho * s.wo;
-  P.num_kblocks = static_cast<int>((P.pixels + 63) / 64);
-  P.total_chunks = s.kh * s.kw * s.cin / 64;
-  P.ntaps_c = s.kh * s.kw;
-  DIRB_CHECK_ARG(stem || P.ntaps_c <= kMaxTaps, "conv_wgrad: at most %d filter taps (got %dx%d)", kMaxTaps, s.kh, s.kw);
-  for (int i = 0; i < kMaxTaps; ++i) P.tap_list[i] = i;
-  const int splits = conv_wgrad_splits(s);
-  P.kblocks_per_split = (P.num_kblocks + splits - 1) / splits;
-  P.ldc = s.cout; P.out = partial;
-  const int bn = wgrad_bn(s);
-  P.n_tiles = s.cout / bn;
-  const int m_tiles = (P.total_chunks + 1) / 2;
-  *splits_out = splits;
-  CUtensorMap tm;
-  if (int rc = make_tmap_bf16_2d(&tm, dy, s.cout, static_cast<uint64_t>(P.pixels), static_cast<uint64_t>(s.cout) * 2, 64))
-    return rc;
-  if (stem) return DISPATCH_BN(bn, true, true, tm, P, m_tiles, splits, st);
-  if (is_plain_gemm(s, stem)) {
-    CUtensorMap ta;     // x as [pixels][cin], 64-pixel x 64-channel boxes
-    if (int rc = make_tmap_bf16_2d(&ta, x, s.cin, static_cast<uint64_t>(P.pixels), static_cast<uint64_t>(s.cin) * 2, 64))
-      return rc;
-    P.a_mode = 1;
-    return DISPATCH_BN(bn, true, false, tm, P, m_tiles, splits, st, &ta);
-  }
-  if (im2col_enabled()) {
-    CUtensorMap ta;     // x [n,h,w,cin]: 64 output positions x 64 channels per load
-    if (int rc = make_tmap_im2col_bf16(&ta, x, s.cin, s.w, s.h, s.n, -s.pad, -s.pad, s.pad - (s.kw - 1),
-                                       s.pad - (s.kh - 1), s.stride, 64))
-      return rc;
-    P.a_mode = 2; P.i2c_stride = s.stride; P.i2c_lo = -s.pad;
-    return DISPATCH_BN(bn, true, false, tm, P, m_tiles, splits, st, &ta);
-  }
-  return DISPATCH_BN(bn, true, false, tm, P, m_tiles, splits, st);
-}
-
-// Host-only description of the launch a conv would get (no CUDA call): which tile width, operand feeding form and
-// split-K factor the selection logic above picks.  op: 0 fprop, 1 dgrad, 2 wgrad.
-// plan[0] = BN, plan[1] = 0 (no CTA pairs in this build), plan[2] = A-operand form (0 cp.async gather, 1 tiled TMA,
-// 2 im2col TMA), plan[3] = 0 (no patch-resident form in this build), plan[4] = split-K factor (wgrad; else 1),
-// plan[5] = launches (stride-2 dgrad: one per non-empty parity class), plan[6] = 1 if the dgrad can carry the BN-backward
-// moments of the previous layer.
-int conv_plan(const ConvShape& s, bool stem, int op, int* plan) {
-  for (int i = 0; i < 7; ++i) plan[i] = 0;
-  plan[4] = plan[5] = 1;
-  if (int rc = check_shape(s, stem, "conv_plan")) return rc;
-  if (op == 2) {
-    plan[0] = wgrad_bn(s);
-    plan[4] = conv_wgrad_splits(s);
-    plan[2] = stem ? 0 : (is_plain_gemm(s, stem) ? 1 : (im2col_enabled() ? 2 : 0));
-    return DIRB200_OK;
-  }
-  const bool dgrad = op == 1;
-  DIRB_CHECK_ARG(!(dgrad && stem), "conv_plan: the stem has no data gradient");
-  const int n_dim = dgrad ? s.cin : s.cout;
-  plan[0] = pick_bn(n_dim);
-  if (dgrad && s.stride == 2) {
-    int launches = 0;
-    for (int cls = 0; cls < 4; ++cls) {
-      const int py = cls >> 1, px = cls & 1;
-      int nt = 0;
-      for (int r = 0; r < s.kh; ++r)
-        for (int q = 0; q < s.kw; ++q)
-          if (((py + s.pad - r) & 1) == 0 && ((px + s.pad - q) & 1) == 0) ++nt;
-      const int hm = (s.h - py + 1) / 2, wm = (s.w - px + 1) / 2;
-      if (nt == 0 || hm <= 0 || wm <= 0) continue;
-      ++launches;
-    }
-    plan[2] = im2col_enabled() ? 2 : 0; plan[5] = launches;
-    return DIRB200_OK;
-  }
-  const bool tma_fed = is_plain_gemm(s, stem) || (!stem && im2col_enabled() && (!dgrad || s.kh == s.kw));
-  plan[2] = stem ? 0 : (is_plain_gemm(s, stem) ? 1 : (tma_fed ? 2 : 0));
-  plan[6] = dgrad && conv_dgrad_fuses_bn_moments(s);
-  return DIRB200_OK;
+  P.src = x; P.out = partial;
+  *splits_out = pl.splits;
+  return run_plan(s, pl, P, dy, st);
 }
 
 }  // namespace dirb200

@@ -26,7 +26,8 @@ struct ConvLayer {
   bool stem = false;
   size_t w_off = 0;
   __nv_bfloat16 *wf = nullptr, *wd = nullptr;  // GEMM operands (fprop / dgrad layouts)
-  float* wpart = nullptr;                      // split-K partials of this layer's weight gradient
+  float* wpart = nullptr;                      // split-K partials of this layer's weight gradient ...
+  int splits = 1;                              // ... their count (the wgrad plan's)
   __nv_bfloat16* y = nullptr;                  // raw conv output [rows][cout]
   __nv_bfloat16* a = nullptr;                  // relu(bn(y)) when this conv is followed by BN+ReLU
   int64_t rows = 0;                            // n*ho*wo
@@ -141,7 +142,10 @@ static bool setup_conv(dirb200_net* net, ConvLayer& cv, int n, int h, int w, int
   const size_t welems = stem ? (size_t)cout * 256 : (size_t)cout * cin * k * k;
   NET_ALLOC(cv.wf, welems * 2);
   if (!stem) NET_ALLOC(cv.wd, welems * 2);
-  NET_ALLOC(cv.wpart, conv_wgrad_workspace_bytes(cv.s));
+  ConvPlan wp;
+  if (plan_conv(cv.s, stem, 2, &wp) != DIRB200_OK) return false;
+  cv.splits = wp.splits;
+  NET_ALLOC(cv.wpart, wp.workspace_bytes);
   NET_ALLOC(cv.y, (size_t)cv.rows * cout * 2);
   if (with_act) NET_ALLOC(cv.a, (size_t)cv.rows * cout * 2);
   return setup_bn(net, cv.bn, cout);
@@ -194,7 +198,7 @@ static bool build(dirb200_net* net, const int* blocks_per_stage, int num_stages)
     // split-K reduction jobs: every conv owns its partial buffer; one launch reduces a whole backward stage
     std::vector<WgradReduceDesc> rd;
     auto addr = [&](const ConvLayer& cv) {
-      rd.push_back(WgradReduceDesc{cv.wpart, cv.w_off, conv_wgrad_splits(cv.s), cv.s.cout, cv.stem ? 3 : cv.s.cin,
+      rd.push_back(WgradReduceDesc{cv.wpart, cv.w_off, cv.splits, cv.s.cout, cv.stem ? 3 : cv.s.cin,
                                    cv.stem ? 7 : cv.s.kh, cv.stem ? 7 : cv.s.kw, cv.stem ? 1 : 0});
     };
     net->reduce_begin.clear();
@@ -494,7 +498,8 @@ static bool fused_bwd_moments() {
 // `prev` come out of the epilogue (*fused = true, *lay = their row layout in net->bn_partial)
 static int dgrad_with_bn_moments(dirb200_net* net, const __nv_bfloat16* dy, ConvLayer& cv, ConvLayer& prev,
                                  __nv_bfloat16* g, StatLayout* lay, bool* fused, cudaStream_t st) {
-  *fused = fused_bwd_moments() && conv_dgrad_fuses_bn_moments(cv.s);
+  ConvPlan pl;
+  *fused = fused_bwd_moments() && plan_conv(cv.s, false, 1, &pl) == DIRB200_OK && pl.fuses_bn_moments;
   if (!*fused) {
     RUNP(kDgrad, conv_dgrad(dy, cv.wd, g, cv.s, st));
     return DIRB200_OK;

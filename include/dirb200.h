@@ -337,7 +337,8 @@ int dirb200_conv_dgrad(const void* dy, const void* w_dgrad, void* dx, int n, int
  * sm_90a); [2] A-operand form: 0 cp.async gather, 1 tiled TMA, 2 im2col-mode TMA; [3] 0 (no patch-resident form on
  * sm_90a); [4] split-K factor (wgrad); [5] launches (a stride-2
  * dgrad runs one per non-empty output-pixel parity class); [6] 1 = this dgrad can also accumulate the BN-backward
- * moments of the previous layer in its epilogue. */
+ * moments of the previous layer in its epilogue.  A shape those entry points would refuse is refused here with the same
+ * status and message. */
 int dirb200_conv_plan(int n, int h, int w, int cin, int cout, int kh, int kw, int stride, int pad, int stem, int op,
                       int* plan7);
 size_t dirb200_conv_wgrad_workspace_bytes(int n, int h, int w, int cin, int cout, int kh, int kw,

@@ -47,7 +47,7 @@ def test_no_cpu_fallback():
 
 
 def test_wgrad_split_search_never_leaves_a_straggler_wave():
-    """Host-side scheduling of the wgrad split-K GEMM (csrc/conv_igemm.cu: conv_wgrad_splits), observable without a
+    """Host-side scheduling of the wgrad split-K GEMM (csrc/conv_igemm.cu: plan_conv), observable without a
     GPU through dirb200_conv_wgrad_workspace_bytes = splits * K_total * Cout * 4, with the SM count the library itself
     uses (num_sms(): the device's, capped by DIRB200_SMS; the H100 SXM's 132 when no device is present).  For every conv of the batch-256 ResNet-50: the work items (tiles x splits) must fill the
     persistent CTAs' waves to >= 85 % -- a ceil(2*SMs/tiles) rule leaves a straggler wave of a few items on the 3x3
@@ -89,16 +89,27 @@ def test_wgrad_split_search_never_leaves_a_straggler_wave():
 
 def test_conv_plan_selects_the_intended_gemm_forms():
     """Host-only selection logic of the conv stage (dirb200_conv_plan; no device needed): the batch-256 ResNet-50 shapes
-    get the forms DESIGN.md section 4 describes."""
+    get the forms DESIGN.md section 4 describes, and the query refuses what a launch refuses."""
     import ctypes
+    import json
+    import subprocess
+    import sys
     import _lib, _convlib  # noqa: F401
 
-    def plan(h, cin, cout, k, s, p, op, stem=0, hw_in=None):
+    def query(h, cin, cout, k, s, p, op, stem=0):
         a = (ctypes.c_int * 7)()
-        hh = hw_in or h
-        rc = _lib.raw("dirb200_conv_plan")(256, hh, hh, cin, cout, k, k, s, p, stem, op, a)
+        rc = _lib.raw("dirb200_conv_plan")(256, h, h, cin, cout, k, k, s, p, stem, op, a)
+        return rc, dict(zip(("bn", "pairs", "feed", "patch_rows", "splits", "launches", "bn_moments"), a))
+
+    def plan(*args, **kw):
+        rc, q = query(*args, **kw)
         assert rc == 0, _lib.last_error()
-        return dict(zip(("bn", "pairs", "feed", "patch_rows", "splits", "launches", "bn_moments"), a))
+        return q
+
+    def refused(*args, msg):
+        rc, _ = query(*args)
+        err = _lib.last_error()
+        assert rc == -1 and msg in err, (args, rc, err)
 
     GATHER, TILED, IM2COL = 0, 1, 2
     # layer1 conv2 (64 -> 64 3x3 at 56x56): im2col TMA, 64-wide tiles in all three passes; its dgrad carries BN moments
@@ -126,6 +137,39 @@ def test_conv_plan_selects_the_intended_gemm_forms():
     # 5x5 (NYUD2 refinement conv) goes through im2col TMA as well; the stem keeps the cp.async gather
     assert plan(240, 128, 128, 5, 1, 2, 0)["feed"] == IM2COL
     assert plan(224, 3, 64, 7, 2, 3, 0, stem=1)["feed"] == GATHER
+    # stride-2 dgrad: one launch per output-pixel parity class (py, px) that has pixels and a filter tap (r, s) with
+    # r = py + pad, s = px + pad (mod 2); on a 1x1 map only the (even, even) class has pixels
+    for k, p, launches in ((1, 0, 1), (1, 1, 1), (3, 0, 4), (3, 1, 4)):
+        assert plan(56, 128, 128, k, 2, p, 1)["launches"] == launches, (k, p)
+    assert plan(1, 128, 128, 3, 2, 1, 1)["launches"] == 1
+    # refusals: more than 25 filter taps; a stride-2 dgrad with more than 9; a dgrad of stride other than 1 or 2
+    for op in (0, 1, 2):
+        refused(14, 64, 64, 7, 1, 3, op, msg="filter taps")
+    assert plan(28, 64, 64, 5, 2, 2, 0)["feed"] == IM2COL
+    refused(28, 64, 64, 5, 2, 2, 1, msg="filter taps")
+    assert plan(28, 64, 64, 3, 3, 1, 0)["feed"] == IM2COL
+    refused(28, 64, 64, 3, 3, 1, 1, msg="stride must be 1 or 2")
+    # the switches are read once per process: DIRB200_ATMA=0 leaves every conv to the cp.async gather,
+    # DIRB200_IM2COL=0 keeps the tiled TMA of the 1x1 stride-1 GEMMs and gathers the rest
+    shapes = [(56, 64, 256, 1, 1, 0), (56, 64, 64, 3, 1, 1), (56, 128, 128, 3, 2, 1), (56, 256, 512, 1, 2, 0),
+              (60, 128, 128, 5, 1, 2)]
+    code = ("import ctypes, json, sys, _lib, _convlib\n"
+            "forms = []\n"
+            "for (h, cin, cout, k, s, p) in json.loads(sys.argv[1]):\n"
+            "    for op in (0, 1, 2):\n"
+            "        a = (ctypes.c_int * 7)()\n"
+            "        assert _lib.raw('dirb200_conv_plan')(256, h, h, cin, cout, k, k, s, p, 0, op, a) == 0, _lib.last_error()\n"
+            "        forms.append(a[2])\n"
+            "print(json.dumps(forms))\n")
+    plain = [1 if (k, s, p) == (1, 1, 0) else 0 for (h, cin, cout, k, s, p) in shapes for op in (0, 1, 2)]
+    assert [plan(*sh, op)["feed"] for sh in shapes for op in (0, 1, 2)] == [TILED if t else IM2COL for t in plain]
+    for var, want in (("DIRB200_ATMA", [GATHER] * len(plain)), ("DIRB200_IM2COL", [TILED if t else GATHER for t in plain])):
+        env = dict(os.environ, **{var: "0"})
+        env["PYTHONPATH"] = os.pathsep.join([os.path.join(ROOT, "imbalanced-regression_b200"), env.get("PYTHONPATH", "")])
+        r = subprocess.run([sys.executable, "-c", code, json.dumps(shapes)], env=env, cwd=ROOT, capture_output=True,
+                           text=True)
+        assert r.returncode == 0, r.stderr
+        assert json.loads(r.stdout.strip().splitlines()[-1]) == want, (var, r.stdout)
 
 
 def test_fused_epilogue_test_aids_refuse_bad_arguments_before_any_cuda_call():

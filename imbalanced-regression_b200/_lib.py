@@ -15,6 +15,7 @@ BIN_AGE, BIN_DEPTH10, BIN_EDGES5 = 0, 1, 2
 LOSS_KINDS = {"mse": 0, "l1": 1, "focal_mse": 2, "focal_l1": 3, "huber": 4}
 ACTIVATE = {"sigmoid": 0, "tanh": 1}
 REWEIGHT = {"sqrt_inv": 1, "inverse": 2}
+DIRB200_ERR_ARG = -1
 
 
 class Dirb200Error(RuntimeError):
@@ -105,6 +106,13 @@ _SIGS = {
     "dirb200_pair_maxpool_fwd": (c_int, [P, P, P, c_int, c_int, c_int, c_int, P, P, P]),
     "dirb200_pair_maxpool_bwd": (c_int, [P, P, P, P, c_int, c_int, c_int, c_int, P, P]),
     "dirb200_stsb_gather_batch": (c_int, [P, P, P, P, c_int64, c_int, P, c_int64, c_int, c_int, P, P, P, P, P]),
+    # JPEG decode + Pillow bilinear resize (csrc/jpeg.cu); the parse and the two size queries are host-only
+    "dirb200_jpeg_desc_bytes": (c_size_t, []),
+    "dirb200_jpeg_parse": (c_int, [P, c_int64, P, P, c_int64]),
+    "dirb200_jpeg_decode_workspace_bytes": (c_size_t, [P, c_int]),
+    "dirb200_jpeg_decode": (c_int, [P, P, P, P, c_int, P, P, P, P, c_size_t, P]),
+    "dirb200_resize_bilinear_workspace_bytes": (c_size_t, [P, c_int, c_int, c_int]),
+    "dirb200_resize_bilinear_u8": (c_int, [P, P, P, c_int, c_int, c_int, P, P, c_size_t, P]),
 }
 
 

@@ -7,6 +7,7 @@ convolution and the per-sample weight gather run in libdirb200
 (PIL decode, crop, flip, normalise; datasets.py:27-53) is out of scope of the
 hot path (SURVEY.md §2a row 8) and kept as thin torchvision host code.
 """
+import io
 import logging
 import os
 
@@ -70,10 +71,13 @@ class AgeDB(data.Dataset):
     label_column = 'age'
 
     def __init__(self, df, data_dir, img_size, split='train', reweight='none',
-                 lds=False, lds_kernel='gaussian', lds_ks=5, lds_sigma=2, device_transform=False):
+                 lds=False, lds_kernel='gaussian', lds_ks=5, lds_sigma=2, device_transform=False, device_decode=False):
         # device_transform (not in the reference): __getitem__ stops after the resize and returns the uint8 HWC image;
-        # the rest of get_transform() runs on the GPU for the whole batch (gpu_transform_batch below)
-        self.device_transform = device_transform
+        # the rest of get_transform() runs on the GPU for the whole batch (gpu_transform_batch below).
+        # device_decode (implies device_transform): __getitem__ returns a JPEG in the device decoder's supported set as
+        # its bytes (EncodedJpeg); jpeg_collate + JpegBatch.cuda() decode and resize the batch on the GPU
+        self.device_transform = device_transform or device_decode
+        self.device_decode = device_decode
         self.df = df
         self.data_dir = data_dir
         self.img_size = img_size
@@ -89,12 +93,17 @@ class AgeDB(data.Dataset):
         from PIL import Image
         index = index % len(self.df)
         row = self.df.iloc[index]
-        img = Image.open(os.path.join(self.data_dir, row['path'])).convert('RGB')
-        if self.device_transform:
-            from torchvision import transforms
-            img = torch.from_numpy(np.asarray(transforms.Resize((self.img_size, self.img_size))(img)).copy())
-        else:
-            img = self.get_transform()(img)
+        path = os.path.join(self.data_dir, row['path'])
+        img = None
+        if self.device_decode:
+            with open(path, 'rb') as f:
+                raw = f.read()
+            rc, desc, intervals = parse_jpeg(raw)
+            if rc == 0:
+                img = EncodedJpeg(raw, desc, intervals, self.img_size)
+        if img is None:
+            img = Image.open(path).convert('RGB')
+            img = host_resize_u8(img, self.img_size) if self.device_transform else self.get_transform()(img)
         label = np.asarray([row[self.label_column]]).astype('float32')
         weight = np.asarray([self.weights[index]]).astype('float32') if self.weights is not None else \
             np.asarray([np.float32(1.)])
@@ -116,6 +125,148 @@ class AgeDB(data.Dataset):
 
 class IMDBWIKI(AgeDB):
     pass
+
+
+def host_resize_u8(img, size):
+    """transforms.Resize((size, size)) of a PIL image as a uint8 HWC tensor: the device_transform sample."""
+    from torchvision import transforms
+    return torch.from_numpy(np.asarray(transforms.Resize((size, size))(img)).copy())
+
+
+# ------------------------------------------------------------------ JPEG decode + resize on the device
+# dirb200_jpeg_desc (include/dirb200.h), field for field
+JPEG_DESC_DTYPE = np.dtype([(k, '<i4') for k in ('height', 'width', 'ncomp', 'hmax', 'vmax', 'mcus_x', 'mcus_y',
+                                                 'restart_interval', 'n_intervals', 'scan_begin', 'scan_end')] +
+                           [(k, '<i4', (3,)) for k in ('comp_h', 'comp_v', 'comp_tq', 'comp_td', 'comp_ta')] +
+                           [('qt', '<u2', (4, 64)), ('huff_bits', 'u1', (2, 4, 16)), ('huff_vals', 'u1', (2, 4, 256))])
+JPEG_DESC_BYTES = int(_lib.raw("dirb200_jpeg_desc_bytes")())
+assert JPEG_DESC_DTYPE.itemsize == JPEG_DESC_BYTES, (JPEG_DESC_DTYPE.itemsize, JPEG_DESC_BYTES)
+
+
+def parse_jpeg(raw):
+    """dirb200_jpeg_parse on one file's bytes (host only, no CUDA call): (rc, desc uint8 [JPEG_DESC_BYTES],
+    intervals int32 [n_intervals]).  rc 0: supported; > 0: not a supported JPEG; < 0: a malformed JPEG."""
+    a = np.frombuffer(raw, dtype=np.uint8)
+    desc = np.zeros(JPEG_DESC_BYTES, dtype=np.uint8)
+    intervals = np.zeros((len(a) + 3) // 2, dtype=np.int32)
+    rc = _lib.raw("dirb200_jpeg_parse")(a.ctypes.data_as(_lib.P) if len(a) else None, len(a),
+                                        desc.ctypes.data_as(_lib.P), intervals.ctypes.data_as(_lib.P), len(intervals))
+    if rc == _lib.DIRB200_ERR_ARG:
+        raise _lib.Dirb200Error(f"dirb200_jpeg_parse: {_lib.last_error()}")
+    n_iv = int(desc.view(JPEG_DESC_DTYPE)[0]['n_intervals']) if rc == 0 else 0
+    return rc, desc, intervals[:n_iv].copy()
+
+
+class EncodedJpeg:
+    """One supported JPEG as AgeDB(device_decode=True) yields it: the file's bytes, its descriptor and restart-interval
+    table, and the square size it is to be resized to."""
+    __slots__ = ('raw', 'desc', 'intervals', 'size')
+
+    def __init__(self, raw, desc, intervals, size):
+        self.raw, self.desc, self.intervals, self.size = raw, desc, intervals, size
+
+    @property
+    def hw(self):
+        d = self.desc.view(JPEG_DESC_DTYPE)[0]
+        return int(d['height']), int(d['width'])
+
+
+_DECODE_STATS = {'device': 0, 'flagged': 0, 'host': 0}
+
+
+def take_device_decode_stats():
+    """Images since the last call: decoded on the device, flagged by it (and decoded by Pillow after the batch's
+    status read), and decoded by Pillow in the loader (outside the supported set)."""
+    out = dict(_DECODE_STATS)
+    for k in _DECODE_STATS:
+        _DECODE_STATS[k] = 0
+    return out
+
+
+class JpegBatch:
+    """A batch of AgeDB(device_decode=True) samples: the supported JPEGs packed for dirb200_jpeg_decode (bytes,
+    offsets, descriptors, interval tables) and the images the loader already decoded and resized, with their batch
+    positions.  .cuda() returns the uint8 [N, S, S, 3] tensor that stacking AgeDB(device_transform=True) items gives."""
+
+    def __init__(self, items):
+        self.n = len(items)
+        self.jpeg_pos = [i for i, it in enumerate(items) if isinstance(it, EncodedJpeg)]
+        self.host_pos = [i for i, it in enumerate(items) if not isinstance(it, EncodedJpeg)]
+        jp = [items[i] for i in self.jpeg_pos]
+        sizes = {it.size for it in jp} | {int(items[i].shape[0]) for i in self.host_pos}
+        assert len(sizes) == 1, f"one image size per batch, got {sorted(sizes)}"
+        self.size = sizes.pop()
+        self.host = torch.stack([items[i] for i in self.host_pos]) if self.host_pos else None
+        self.raw_lengths = [len(it.raw) for it in jp]
+        lens = np.asarray(self.raw_lengths, dtype=np.int64)
+        self.offsets = torch.from_numpy(np.concatenate([[0], np.cumsum(lens)]).astype(np.int64))
+        self.data = torch.from_numpy(np.frombuffer(b''.join(it.raw for it in jp), dtype=np.uint8).copy())
+        descs = np.stack([it.desc for it in jp]) if jp else np.zeros((0, JPEG_DESC_BYTES), np.uint8)
+        self.descs = torch.from_numpy(descs)
+        self.intervals = torch.from_numpy(np.concatenate([it.intervals for it in jp]) if jp else np.zeros(0, np.int32))
+        hw = np.asarray([it.hw for it in jp], dtype=np.int32).reshape(-1, 2)
+        self.hw = torch.from_numpy(hw)
+        self.rgb_offsets = torch.from_numpy(np.concatenate([[0], np.cumsum(hw[:, 0].astype(np.int64) * hw[:, 1] * 3)])
+                                            .astype(np.int64))
+        m = len(jp)
+        self.decode_ws = int(_lib.raw("dirb200_jpeg_decode_workspace_bytes")(descs.ctypes.data_as(_lib.P), m)) if m else 0
+        self.resize_ws = int(_lib.raw("dirb200_resize_bilinear_workspace_bytes")(
+            hw.ctypes.data_as(_lib.P), m, self.size, self.size)) if m else 0
+        self.flagged = None
+
+    def pin_memory(self):
+        for k in ('data', 'offsets', 'descs', 'intervals', 'hw', 'rgb_offsets', 'host'):
+            t = getattr(self, k)
+            if t is not None and t.numel():
+                setattr(self, k, t.pin_memory())
+        return self
+
+    def _host_decode(self, j):
+        from PIL import Image
+        lo = int(self.offsets[j])
+        raw = self.data[lo:lo + self.raw_lengths[j]].numpy().tobytes()
+        return host_resize_u8(Image.open(io.BytesIO(raw)).convert('RGB'), self.size)
+
+    def cuda(self, device=None, non_blocking=False):
+        dev = torch.device('cuda', torch.cuda.current_device()) if device is None else torch.device(device)
+        S, m = self.size, len(self.jpeg_pos)
+        out = torch.empty(self.n, S, S, 3, dtype=torch.uint8, device=dev)
+        if self.host is not None:
+            out[torch.tensor(self.host_pos, device=dev)] = self.host.to(dev, non_blocking=non_blocking)
+        self.flagged = []
+        if m:
+            up = lambda t: t.to(dev, non_blocking=non_blocking)
+            data, offsets, descs, intervals, hw, rgb_offsets = map(up, (self.data, self.offsets, self.descs,
+                                                                       self.intervals, self.hw, self.rgb_offsets))
+            rgb = torch.empty(int(self.rgb_offsets[-1]), dtype=torch.uint8, device=dev)
+            status = torch.empty(m, dtype=torch.int32, device=dev)
+            ws = torch.empty(self.decode_ws, dtype=torch.uint8, device=dev)
+            st = _lib.stream_ptr()
+            _lib.call("dirb200_jpeg_decode", _lib.ptr(data), _lib.ptr(offsets), _lib.ptr(descs), _lib.ptr(intervals), m,
+                      _lib.ptr(rgb), _lib.ptr(rgb_offsets), _lib.ptr(status), _lib.ptr(ws), ws.numel(), st)
+            dst = out if m == self.n else torch.empty(m, S, S, 3, dtype=torch.uint8, device=dev)
+            rws = torch.empty(self.resize_ws, dtype=torch.uint8, device=dev)
+            _lib.call("dirb200_resize_bilinear_u8", _lib.ptr(rgb), _lib.ptr(rgb_offsets), _lib.ptr(hw), m, S, S,
+                      _lib.ptr(dst), _lib.ptr(rws), rws.numel(), st)
+            if dst is not out:
+                out[torch.tensor(self.jpeg_pos, device=dev)] = dst
+            # the batch's one host sync: images the device flagged are decoded again by Pillow, so their pixels,
+            # warnings and exceptions are Pillow's
+            self.flagged = torch.nonzero(status.cpu()).flatten().tolist()
+            for j in self.flagged:
+                out[self.jpeg_pos[j]] = self._host_decode(j).to(dev)
+        _DECODE_STATS['device'] += m - len(self.flagged)
+        _DECODE_STATS['flagged'] += len(self.flagged)
+        _DECODE_STATS['host'] += len(self.host_pos)
+        return out
+
+
+def jpeg_collate(batch):
+    """collate_fn for AgeDB(device_decode=True): (JpegBatch, labels, weights), the labels and weights collated as the
+    default collate does."""
+    from torch.utils.data import default_collate
+    labels, weights = default_collate([b[1:] for b in batch])
+    return JpegBatch([b[0] for b in batch]), labels, weights
 
 
 # ------------------------------------------------------------------ dense (NYUD2) LDS weights
@@ -202,9 +353,10 @@ def stsb_prepare_weights(scores, reweight, lds=False, lds_kernel='gaussian', lds
 
 # ---------------------------------------------------------------------------------------------------------------------
 # Input pipeline on the device (SURVEY section 8f-4).  The reference transforms every sample on the host, one PIL image
-# at a time (datasets.py:38-53); here the decode + resize stay where they are, and everything after the resize --
-# RandomCrop(img_size, padding=16), RandomHorizontalFlip, ToTensor, Normalize -- runs as ONE kernel over the batch of
-# uint8 images (a quarter of the bytes of the fp32 tensor cross PCIe).
+# at a time (datasets.py:38-53).  Here everything after the resize -- RandomCrop(img_size, padding=16),
+# RandomHorizontalFlip, ToTensor, Normalize -- runs as ONE kernel over the batch of uint8 images (a quarter of the bytes
+# of the fp32 tensor cross PCIe).  With device_decode the JPEG decode and the resize run on the device too (JpegBatch
+# above); images outside the decoder's supported set are decoded and resized on the host in the loader.
 def draw_augment_params(n, size, pad=16, generator=None):
     """The random draws of RandomCrop(size, padding=pad) + RandomHorizontalFlip() for n samples, consumed from the torch
     generator in exactly the order the reference's per-sample Compose does (crop row, crop column, flip coin), so that

@@ -30,7 +30,7 @@ from torch.utils.data import DataLoader, Dataset
 
 from resnet import resnet50
 from loss import *  # noqa: F401,F403  (looked up by name, as the reference does at train.py:255)
-from datasets import AgeDB, IMDBWIKI, gpu_transform_batch, lds_prepare_weights
+from datasets import AgeDB, IMDBWIKI, gpu_transform_batch, jpeg_collate, lds_prepare_weights, take_device_decode_stats
 from utils import AverageMeter, ProgressMeter, adjust_learning_rate, nvtx_range, prepare_folders, save_checkpoint
 from optim import FusedAdam, FusedSGD
 from parallel import DataParallel, ShardSampler, is_distributed
@@ -79,6 +79,10 @@ def build_parser():
     p.add_argument('--device_transform', action='store_true', default=False,
                    help='(not a reference flag) the dataset yields the resized uint8 image; crop / flip / ToTensor / '
                         'Normalize (datasets.py:38-53) run on the GPU for the whole batch (datasets.gpu_transform_batch)')
+    p.add_argument('--device_decode', action='store_true', default=False,
+                   help='(not a reference flag; implies --device_transform) the JPEG decode and Resize((img_size, '
+                        'img_size)) run on the GPU per batch too (datasets.JpegBatch); files outside the device '
+                        "decoder's supported set are decoded by Pillow in the loader")
     return p
 
 
@@ -257,6 +261,7 @@ def validate(val_loader, model, train_labels=None, prefix='Val'):
 
 def main(argv=None):
     args, _ = build_parser().parse_known_args(argv)
+    args.device_transform = args.device_transform or args.device_decode
     args.start_epoch, args.best_loss = 0, 1e5
     args.store_name = store_name(args)
     rank = int(os.environ.get("RANK", "0"))
@@ -287,14 +292,15 @@ def main(argv=None):
         df = pd.read_csv(os.path.join(args.data_dir, f"{args.dataset}.csv"))
         cls = AgeDB if args.dataset == 'agedb' else IMDBWIKI
         parts = {s: df[df['split'] == s] for s in ('train', 'val', 'test')}
-        dt = dict(device_transform=args.device_transform)
+        dt = dict(device_transform=args.device_transform, device_decode=args.device_decode)
         train_dataset = cls(data_dir=args.data_dir, df=parts['train'], img_size=args.img_size, split='train',
                             reweight=args.reweight, lds=args.lds, lds_kernel=args.lds_kernel, lds_ks=args.lds_ks,
                             lds_sigma=args.lds_sigma, **dt)
         val_dataset = cls(data_dir=args.data_dir, df=parts['val'], img_size=args.img_size, split='val', **dt)
         test_dataset = cls(data_dir=args.data_dir, df=parts['test'], img_size=args.img_size, split='test', **dt)
     mk = lambda ds, sampler: DataLoader(ds, batch_size=args.batch_size, sampler=sampler, shuffle=False,
-                                        num_workers=args.workers, pin_memory=True, drop_last=False)
+                                        num_workers=args.workers, pin_memory=True, drop_last=False,
+                                        collate_fn=jpeg_collate if args.device_decode else None)
     n_train = len(train_dataset)
     train_loader = mk(train_dataset, ShardSampler(n_train, rank, world, shuffle=True, pad=True))
     stats_loader = train_loader if world == 1 else mk(train_dataset, ShardSampler(n_train, rank, world, shuffle=False,
@@ -353,6 +359,10 @@ def main(argv=None):
                                    'state_dict': model.state_dict(), 'optimizer': optimizer.state_dict()}, is_best)
         print(f"Epoch #{epoch}: Train loss [{train_loss:.4f}]; Val loss: MSE [{val_mse:.4f}], L1 [{val_l1:.4f}], "
               f"G-Mean [{val_gmean:.4f}]")
+        if args.device_decode:
+            st = take_device_decode_stats()
+            print(f"Epoch #{epoch}: images decoded on the device {st['device']}, flagged by it and decoded by Pillow "
+                  f"{st['flagged']}, outside its supported set (decoded by Pillow in the loader) {st['host']}")
     if is_distributed():
         torch.distributed.destroy_process_group()
 

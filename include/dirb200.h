@@ -233,6 +233,64 @@ int dirb200_depth_head_wgrad(const void* x, const float* dy, float* dw, float* d
 int dirb200_augment_batch(const uint8_t* images, const int* crop_yx, const uint8_t* flip, int n, int size, int pad,
                           float mean, float stdv, float* out, void* stream);
 
+/* JPEG decode and Pillow's bilinear resize on the device (csrc/jpeg.cu): the two host stages of
+ * agedb-dir/datasets.py:30 (Image.open(...).convert('RGB')) and :41 / :49 (transforms.Resize((img_size, img_size))) for a
+ * whole batch, byte for byte as Pillow with libjpeg-turbo produces them.
+ *
+ * dirb200_jpeg_parse (host only, no CUDA call) walks the markers of one file and fills a descriptor.  Returns
+ *   0                          the image is in the supported set below;
+ *   DIRB200_JPEG_UNSUPPORTED   anything else, non-JPEG files included: decode it on the host;
+ *   DIRB200_JPEG_MALFORMED     a malformed or truncated JPEG (the host decoder reports what is wrong with it);
+ *   DIRB200_ERR_ARG            NULL pointers, nbytes outside [0, 2^31) or fewer than n_intervals slots.
+ * Supported: SOF0 / SOF1 (baseline or extended sequential Huffman), 8-bit samples, one scan carrying every component
+ * in frame order, no DNL; 1 component (1 x 1), or 3 components that libjpeg's default colour-space rule takes as
+ * YCbCr (JFIF marker; else an Adobe marker with transform != 0; else component IDs other than 'R', 'G', 'B') with
+ * chroma 1 x 1 and luma 1 x 1, 2 x 1 or 2 x 2; every table the scan uses defined in the file; at most 2^26 pixels.
+ * No byte outside [0, nbytes) is read.  Every Huffman table the scan uses is checked as libjpeg's
+ * jpeg_make_d_derived_tbl checks it.  intervals_host int32 [max_intervals] receives the byte offset at which each
+ * restart interval's entropy-coded data starts (one interval without DRI); (nbytes + 3) / 2 slots always suffice. */
+#define DIRB200_JPEG_UNSUPPORTED 1
+#define DIRB200_JPEG_MALFORMED (-4)
+typedef struct dirb200_jpeg_desc {
+  int32_t height, width;
+  int32_t ncomp;                   /* 1 (grayscale) or 3 (YCbCr) */
+  int32_t hmax, vmax;              /* largest sampling factors (the luma component's) */
+  int32_t mcus_x, mcus_y;          /* MCU grid: ceil(width / (8 hmax)) x ceil(height / (8 vmax)) */
+  int32_t restart_interval;        /* MCUs per restart interval, 0: no DRI */
+  int32_t n_intervals;             /* entries of the interval table (1 without DRI) */
+  int32_t scan_begin, scan_end;    /* [begin, end): the entropy-coded segment, restart markers included */
+  int32_t comp_h[3], comp_v[3];    /* sampling factors per component */
+  int32_t comp_tq[3];              /* quantisation table per component */
+  int32_t comp_td[3], comp_ta[3];  /* DC / AC Huffman table per component (from the SOS header) */
+  uint16_t qt[4][64];              /* DQT values, natural (row-major) order */
+  uint8_t huff_bits[2][4][16];     /* DHT BITS: [0 DC, 1 AC][table][code length - 1] */
+  uint8_t huff_vals[2][4][256];    /* DHT HUFFVAL */
+} dirb200_jpeg_desc;
+size_t dirb200_jpeg_desc_bytes(void);
+int dirb200_jpeg_parse(const uint8_t* data_host, int64_t nbytes, dirb200_jpeg_desc* desc_host, int32_t* intervals_host,
+                       int64_t max_intervals);
+/* Decode n parsed images to RGB u8 HWC, each equal to np.asarray(Image.open(f).convert('RGB')) for the same bytes.
+ * data: the files packed back to back, image b at [offsets[b], offsets[b + 1]) (offsets int64 [n + 1]); descs [n]
+ * from dirb200_jpeg_parse; intervals int32: the images' interval tables concatenated in batch order; rgb_out: image b
+ * at [rgb_offsets[b], rgb_offsets[b + 1]) (int64 [n + 1]), which must hold height * width * 3 bytes.
+ * status int32 [n] (written): 0, or nonzero where the device found an anomaly -- a descriptor outside the supported
+ * set or its byte range, a code not in a Huffman table, entropy data running out, more than 64 coefficients in a
+ * block -- or the workspace is too small.  Such an image's pixels are unspecified: decode it on the host.  No kernel
+ * reads outside an image's byte range or writes outside its output slice.  Stages: Huffman tables, entropy decode
+ * (one thread per restart interval), dequantisation + libjpeg's JDCT_ISLOW IDCT, libjpeg-turbo's fancy upsampling and
+ * YCbCr -> RGB.  The workspace holds the int16 coefficients and the component planes (192 bytes per 8 x 8 block). */
+size_t dirb200_jpeg_decode_workspace_bytes(const dirb200_jpeg_desc* descs_host, int n);
+int dirb200_jpeg_decode(const uint8_t* data, const int64_t* offsets, const dirb200_jpeg_desc* descs,
+                        const int32_t* intervals, int n, uint8_t* rgb_out, const int64_t* rgb_offsets, int32_t* status,
+                        void* workspace, size_t workspace_bytes, void* stream);
+/* Pillow's Image.resize((out_w, out_h), BILINEAR) of n RGB u8 HWC images of mixed sizes, byte for byte: image b
+ * (hw int32 [n][2] = (height, width)) at in + in_offsets[b] (int64 [n]) -> out u8 [n][out_h][out_w][3].  The
+ * workspace holds each image's fixed-point filter coefficients; its size comes from the same sizes on the host.  An
+ * image with a non-positive size, or a call whose workspace does not hold the coefficients, gets zeros. */
+size_t dirb200_resize_bilinear_workspace_bytes(const int32_t* hw_host, int n, int out_h, int out_w);
+int dirb200_resize_bilinear_u8(const uint8_t* in, const int64_t* in_offsets, const int32_t* hw, int n, int out_h,
+                               int out_w, uint8_t* out, void* workspace, size_t workspace_bytes, void* stream);
+
 /* Batched device form of NYUD2-DIR's per-sample chains after Scale(240) (nyud2-dir/loaddata.py:108-125 training,
  * :132-148 FDS, :151-170 test, with nyud2-dir/nyu_transform.py), plus _get_weights (loaddata.py:58-67).
  * images u8 [n][h][w][3] (RGB, HWC); depths u8 [n][h][w] (depth_u16 = 0) or u16 [n][h][w] (depth_u16 = 1: the test

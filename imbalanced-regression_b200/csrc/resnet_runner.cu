@@ -1,4 +1,4 @@
-// Native runner of the bottleneck-ResNet backbone (agedb-dir/resnet.py:41-70,73-138): sequences the
+// Native runner of the ResNet backbone (agedb-dir/resnet.py:14-38 BasicBlock, 41-70 Bottleneck, 73-138): sequences the
 // wgmma convolutions and the HBM-bound layers for one forward and one backward pass over a fixed
 // batch shape, owning every activation / gradient / operand buffer (NHWC bf16) so that a training
 // step issues no allocation and no host synchronisation.
@@ -35,11 +35,17 @@ struct ConvLayer {
 };
 
 struct Block {
-  ConvLayer c1, c2, c3, ds;
+  ConvLayer c1, c2, c3, ds;    // a basic block has no c3
+  bool basic = false;
   bool has_ds = false;
   const __nv_bfloat16* in = nullptr;
   __nv_bfloat16* out = nullptr;
   uint8_t* mask = nullptr;     // ReLU mask of `out`, 1 bit per element ([rows][c/8] bytes), for the backward pass
+  // the tail conv, whose BN output meets the shortcut (bottleneck: conv3, basic block: conv2), and the conv whose
+  // activation it reads (conv2 / conv1)
+  ConvLayer& tail() { return basic ? c2 : c3; }
+  const ConvLayer& tail() const { return basic ? c2 : c3; }
+  ConvLayer& pre_tail() { return basic ? c1 : c2; }
 };
 
 }  // namespace dirb200
@@ -48,6 +54,7 @@ using namespace dirb200;
 
 struct dirb200_net {
   int n = 0, h = 0, w = 0;
+  int block = DIRB200_RESNET_BOTTLENECK;
   ConvLayer stem;
   std::vector<Block> blocks;
   __nv_bfloat16 *x_s2d = nullptr, *pool_out = nullptr;
@@ -167,27 +174,39 @@ static bool build(dirb200_net* net, const int* blocks_per_stage, int num_stages)
   const __nv_bfloat16* cur = net->pool_out;
   size_t max_act = (size_t)net->stem.rows * 64;
   net->stage_begin.assign(1, 0);
+  const bool basic = net->block == DIRB200_RESNET_BASIC;
   for (int st = 0; st < num_stages; ++st) {
     const int planes = 64 << st;
+    const int outc = basic ? planes : planes * 4;    // planes * block.expansion
     net->stage_begin.push_back((int)net->blocks.size());
     for (int b = 0; b < blocks_per_stage[st]; ++b) {
       const int stride = (b == 0 && st > 0) ? 2 : 1;
       net->blocks.emplace_back();
       Block& B = net->blocks.back();
       B.in = cur;
-      B.has_ds = (b == 0) && (stride != 1 || inplanes != planes * 4);
-      if (!setup_conv(net, B.c1, n, h, w, inplanes, planes, 1, 1, 0, false, true)) return false;
-      if (!setup_conv(net, B.c2, n, h, w, planes, planes, 3, stride, 1, false, true)) return false;
-      const int h2 = B.c2.s.ho, w2 = B.c2.s.wo;
-      if (!setup_conv(net, B.c3, n, h2, w2, planes, planes * 4, 1, 1, 0, false, false)) return false;
-      if (B.has_ds && !setup_conv(net, B.ds, n, h, w, inplanes, planes * 4, 1, stride, 0, false, false)) return false;
-      NET_ALLOC(B.out, (size_t)B.c3.rows * planes * 4 * 2);
-      NET_ALLOC(B.mask, (size_t)B.c3.rows * planes * 4 / 8);
-      max_act = std::max(max_act, (size_t)B.c1.rows * std::max(inplanes, planes));
-      max_act = std::max(max_act, (size_t)B.c3.rows * planes * 4);
+      B.basic = basic;
+      B.has_ds = (b == 0) && (stride != 1 || inplanes != outc);
+      // named_parameters() order: conv1, bn1, conv2, bn2[, conv3, bn3], downsample
+      if (basic) {
+        // conv1 3x3 with the stride, conv2 3x3 (agedb-dir/resnet.py:14-38)
+        if (!setup_conv(net, B.c1, n, h, w, inplanes, planes, 3, stride, 1, false, true)) return false;
+        if (!setup_conv(net, B.c2, n, B.c1.s.ho, B.c1.s.wo, planes, planes, 3, 1, 1, false, false)) return false;
+      } else {
+        if (!setup_conv(net, B.c1, n, h, w, inplanes, planes, 1, 1, 0, false, true)) return false;
+        if (!setup_conv(net, B.c2, n, h, w, planes, planes, 3, stride, 1, false, true)) return false;
+        if (!setup_conv(net, B.c3, n, B.c2.s.ho, B.c2.s.wo, planes, outc, 1, 1, 0, false, false)) return false;
+      }
+      const ConvLayer& T = B.tail();
+      if (B.has_ds && !setup_conv(net, B.ds, n, h, w, inplanes, outc, 1, stride, 0, false, false)) return false;
+      NET_ALLOC(B.out, (size_t)T.rows * outc * 2);
+      NET_ALLOC(B.mask, (size_t)T.rows * outc / 8);
+      // the scratch buffers hold any block input / conv output and their gradients
+      max_act = std::max(max_act, (size_t)n * h * w * std::max(inplanes, planes));
+      max_act = std::max(max_act, (size_t)B.c1.rows * planes);
+      max_act = std::max(max_act, (size_t)T.rows * outc);
       cur = B.out;
-      inplanes = planes * 4;
-      h = h2; w = w2;
+      inplanes = outc;
+      h = T.s.ho; w = T.s.wo;
     }
   }
   net->stage_begin.push_back((int)net->blocks.size());
@@ -208,7 +227,8 @@ static bool build(dirb200_net* net, const int* blocks_per_stage, int num_stages)
       net->reduce_begin.push_back((int)rd.size());
       for (int bi = net->stage_begin[stg]; bi < net->stage_begin[stg + 1]; ++bi) {
         Block& B = net->blocks[bi];
-        addr(B.c1); addr(B.c2); addr(B.c3);
+        addr(B.c1); addr(B.c2);
+        if (!B.basic) addr(B.c3);
         if (B.has_ds) addr(B.ds);
       }
     }
@@ -228,7 +248,8 @@ static bool build(dirb200_net* net, const int* blocks_per_stage, int num_stages)
   };
   add(net->stem);
   for (Block& B : net->blocks) {
-    add(B.c1); add(B.c2); add(B.c3);
+    add(B.c1); add(B.c2);
+    if (!B.basic) add(B.c3);
     if (B.has_ds) add(B.ds);
   }
   net->num_convs = (int)descs.size();
@@ -242,7 +263,8 @@ static bool build(dirb200_net* net, const int* blocks_per_stage, int num_stages)
   };
   addbn(net->stem.bn);
   for (Block& B : net->blocks) {
-    addbn(B.c1.bn); addbn(B.c2.bn); addbn(B.c3.bn);
+    addbn(B.c1.bn); addbn(B.c2.bn);
+    if (!B.basic) addbn(B.c3.bn);
     if (B.has_ds) addbn(B.ds.bn);
   }
   net->num_bns = (int)bd.size();
@@ -361,7 +383,7 @@ static int conv_bn_backward(dirb200_net* net, ConvLayer& cv, const __nv_bfloat16
 
 // Inference forward (agedb-dir/train.py:286-335 validate(); resnet.py:46-66,128-138 under model.eval()): BatchNorm uses
 // the running statistics, so it is a per-channel affine map that folds into the conv epilogue -- every
-// conv -> BN [-> ReLU] and the whole conv3 -> BN -> (+ shortcut) -> ReLU tail of a block is ONE launch, and no raw conv
+// conv -> BN [-> ReLU] and the whole tail conv -> BN -> (+ shortcut) -> ReLU of a block is ONE launch, and no raw conv
 // output is written.  ~58 launches instead of ~165.  DIRB200_FOLDED_EVAL=0 keeps the unfused sequence (A/B checks).
 static bool folded_eval() {
   static const bool on = [] {
@@ -381,13 +403,15 @@ static int forward_eval_folded(dirb200_net* net, const float* params, const floa
                                   net->stem.s.wo, 64, net->pool_out, net->pool_idx, st));
   for (Block& B : net->blocks) {
     RUNP(kFprop, conv_fprop_affine(B.in, B.c1.wf, B.c1.a, B.c1.s, ConvEpilogue{B.c1.bn.scale, B.c1.bn.shift, nullptr, true}, st));
-    RUNP(kFprop, conv_fprop_affine(B.c1.a, B.c2.wf, B.c2.a, B.c2.s, ConvEpilogue{B.c2.bn.scale, B.c2.bn.shift, nullptr, true}, st));
+    if (!B.basic)
+      RUNP(kFprop, conv_fprop_affine(B.c1.a, B.c2.wf, B.c2.a, B.c2.s, ConvEpilogue{B.c2.bn.scale, B.c2.bn.shift, nullptr, true}, st));
     const __nv_bfloat16* shortcut = B.in;
     if (B.has_ds) {
       RUNP(kFprop, conv_fprop_affine(B.in, B.ds.wf, B.ds.y, B.ds.s, ConvEpilogue{B.ds.bn.scale, B.ds.bn.shift, nullptr, false}, st));
       shortcut = B.ds.y;
     }
-    RUNP(kFprop, conv_fprop_affine(B.c2.a, B.c3.wf, B.out, B.c3.s, ConvEpilogue{B.c3.bn.scale, B.c3.bn.shift, shortcut, true}, st));
+    ConvLayer& T = B.tail();
+    RUNP(kFprop, conv_fprop_affine(B.pre_tail().a, T.wf, B.out, T.s, ConvEpilogue{T.bn.scale, T.bn.shift, shortcut, true}, st));
   }
   if (enc_out) RUNP(kPool, avgpool_fwd(net->blocks.back().out, net->n, net->feat_hw, net->feat_c, enc_out, st));
   return DIRB200_OK;
@@ -402,15 +426,16 @@ static int forward_body(dirb200_net* net, const float* params, float* running, b
                                   net->stem.s.wo, 64, net->pool_out, net->pool_idx, st));
   for (Block& B : net->blocks) {
     RUN(conv_bn_forward(net, B.c1, B.in, params, running, tr, st));
-    RUN(conv_bn_forward(net, B.c2, B.c1.a, params, running, tr, st));
-    RUN(conv_bn_forward(net, B.c3, B.c2.a, params, running, tr, st));
+    if (!B.basic) RUN(conv_bn_forward(net, B.c2, B.c1.a, params, running, tr, st));
+    ConvLayer& T = B.tail();
+    RUN(conv_bn_forward(net, T, B.pre_tail().a, params, running, tr, st));     // T.a == nullptr: no bn_apply
     if (B.has_ds) {
       RUN(conv_bn_forward(net, B.ds, B.in, params, running, tr, st));
-      RUNP(kBnApply, bn_apply(B.c3.y, B.c3.bn.scale, B.c3.bn.shift, nullptr, B.ds.y, B.ds.bn.scale, B.ds.bn.shift, true,
-                              B.c3.rows, B.c3.bn.c, B.out, tr ? B.mask : nullptr, st));
+      RUNP(kBnApply, bn_apply(T.y, T.bn.scale, T.bn.shift, nullptr, B.ds.y, B.ds.bn.scale, B.ds.bn.shift, true,
+                              T.rows, T.bn.c, B.out, tr ? B.mask : nullptr, st));
     } else {
-      RUNP(kBnApply, bn_apply(B.c3.y, B.c3.bn.scale, B.c3.bn.shift, B.in, nullptr, nullptr, nullptr, true, B.c3.rows,
-                              B.c3.bn.c, B.out, tr ? B.mask : nullptr, st));
+      RUNP(kBnApply, bn_apply(T.y, T.bn.scale, T.bn.shift, B.in, nullptr, nullptr, nullptr, true, T.rows,
+                              T.bn.c, B.out, tr ? B.mask : nullptr, st));
     }
   }
   if (enc_out) RUNP(kPool, avgpool_fwd(net->blocks.back().out, net->n, net->feat_hw, net->feat_c, enc_out, st));
@@ -418,7 +443,7 @@ static int forward_body(dirb200_net* net, const float* params, float* running, b
 }
 
 // Multi-scale mode hands out (and takes a gradient for) the output of the last block of every layer group; that block
-// must be an identity block (true of every layer group of ResNet-50 and deeper), whose output BN-backward reduction
+// must be an identity block (true of every layer group of ResNet-18 and deeper), whose output BN-backward reduction
 // takes the group's gradient as a third operand.
 static int check_blocks_mode(const dirb200_net* net, const char* who) {
   const int nst = (int)net->stage_begin.size() - 2;
@@ -518,6 +543,13 @@ static constexpr int kMaxNetSide = 2 * (1 << 9);    // stem-output row / column:
 extern "C" {
 
 int dirb200_resnet_create(int n, int h, int w, const int* blocks_per_stage, int num_stages, dirb200_net** out) {
+  return dirb200_resnet_create_ex(n, h, w, DIRB200_RESNET_BOTTLENECK, blocks_per_stage, num_stages, out);
+}
+
+int dirb200_resnet_create_ex(int n, int h, int w, int block, const int* blocks_per_stage, int num_stages,
+                             dirb200_net** out) {
+  DIRB_CHECK_ARG(block == DIRB200_RESNET_BOTTLENECK || block == DIRB200_RESNET_BASIC,
+                 "resnet_create: bad block kind %d (0 bottleneck, 1 basic)", block);
   DIRB_CHECK_ARG(out && blocks_per_stage && n > 0 && num_stages >= 1 && num_stages <= 4, "resnet_create: bad arguments");
   // the input space-to-depth needs even H and W, the max-pool backward an even stem output (H/2, W/2)
   DIRB_CHECK_ARG(h > 0 && w > 0 && h % 4 == 0 && w % 4 == 0, "resnet_create: H and W must be multiples of 4 (got %dx%d)",
@@ -532,6 +564,7 @@ int dirb200_resnet_create(int n, int h, int w, const int* blocks_per_stage, int 
                  "resnet_create: N * H/2 * W/2 must be below 2^31 (got %d x %d x %d)", n, h / 2, w / 2);
   dirb200_net* net = new dirb200_net();
   net->n = n; net->h = h; net->w = w;
+  net->block = block;
   if (!build(net, blocks_per_stage, num_stages)) {
     for (void* p : net->allocs) cudaFree(p);
     delete net;
@@ -640,7 +673,7 @@ int dirb200_resnet_forward_blocks(dirb200_net* net, const float* x_nchw, const f
   }
   for (int s = 0; s < nst; ++s) {
     const Block& B = net->blocks[net->stage_begin[s + 2] - 1];
-    DIRB_CUDA(cudaMemcpyAsync(block_out[s], B.out, sizeof(__nv_bfloat16) * (size_t)B.c3.rows * B.c3.s.cout,
+    DIRB_CUDA(cudaMemcpyAsync(block_out[s], B.out, sizeof(__nv_bfloat16) * (size_t)B.tail().rows * B.tail().s.cout,
                               cudaMemcpyDeviceToDevice, st));
   }
   net->forward_was_training = tr;
@@ -660,40 +693,44 @@ static int backward_blocks(dirb200_net* net, int lo, int hi, const float* params
   int gB_h = net->bw_gB_h, gB_w = net->bw_gB_w;
   for (int bi = hi - 1; bi >= lo; --bi) {
     Block& B = net->blocks[bi];
-    BNLayer& b3 = B.c3.bn;
-    // ---- block output: out = relu(bn3(y3) + identity); dz = (gA + gB) * (out > 0)
+    ConvLayer& T = B.tail();       // conv3 (bottleneck) / conv2 (basic block)
+    ConvLayer& M = B.pre_tail();   // the conv whose activation T reads: conv2 / conv1
+    BNLayer& b3 = T.bn;
+    // ---- block output: out = relu(bn_T(y_T) + identity); dz = (gA + gB) * (out > 0)
     int nblk = 0;
     const int kparts = B.has_ds ? 3 : 2;
     // identity blocks: the reduction also stores dz (= the gradient of the shortcut path, nB) so that the apply pass
     // reads ONE gradient tensor instead of gA, gB and the mask again
-    RUNP(kBnBwdReduce, bn_bwd_reduce(gA, gB, B.c3.y, B.has_ds ? B.ds.y : nullptr, nullptr, nullptr, B.mask, B.c3.rows,
+    RUNP(kBnBwdReduce, bn_bwd_reduce(gA, gB, T.y, B.has_ds ? B.ds.y : nullptr, nullptr, nullptr, B.mask, T.rows,
                                      b3.c, net->bn_partial, &nblk, st, gB_h, gB_w, B.has_ds ? nullptr : nB,
                                      bi == hi - 1 ? g3 : nullptr));
     if (B.has_ds) {
       BNLayer& bd = B.ds.bn;
-      RUNP(kBnBwdApply, bn_bwd_coeffs(net->bn_partial, nblk, kparts, 2, B.c3.rows, b3.c, bd.mean, bd.invstd,
+      RUNP(kBnBwdApply, bn_bwd_coeffs(net->bn_partial, nblk, kparts, 2, T.rows, b3.c, bd.mean, bd.invstd,
                                       params + bd.gamma_off, grads + bd.gamma_off, grads + bd.beta_off, bd.coef, st));
     }
-    RUNP(kBnBwdApply, bn_bwd_coeffs(net->bn_partial, nblk, kparts, 1, B.c3.rows, b3.c, b3.mean, b3.invstd,
+    RUNP(kBnBwdApply, bn_bwd_coeffs(net->bn_partial, nblk, kparts, 1, T.rows, b3.c, b3.mean, b3.invstd,
                                     params + b3.gamma_off, grads + b3.gamma_off, grads + b3.beta_off, b3.coef, st));
     if (B.has_ds)
-      RUNP(kBnBwdApply, bn_bwd_apply(gA, gB, B.c3.y, b3.coef, B.ds.y, B.ds.bn.coef, nullptr, nullptr, B.mask, B.c3.rows,
+      RUNP(kBnBwdApply, bn_bwd_apply(gA, gB, T.y, b3.coef, B.ds.y, B.ds.bn.coef, nullptr, nullptr, B.mask, T.rows,
                                      b3.c, t1, t2, nullptr, st, gB_h, gB_w));
     else
-      RUNP(kBnBwdApply, bn_bwd_apply(nB, nullptr, B.c3.y, b3.coef, nullptr, nullptr, nullptr, nullptr, nullptr, B.c3.rows,
+      RUNP(kBnBwdApply, bn_bwd_apply(nB, nullptr, T.y, b3.coef, nullptr, nullptr, nullptr, nullptr, nullptr, T.rows,
                                      b3.c, t1, nullptr, nullptr, st));
     gB_h = gB_w = 0;
-    // ---- conv3
-    RUN(wgrad_step(net, B.c2.a, t1, B.c3, st));
+    // ---- tail conv
+    RUN(wgrad_step(net, M.a, t1, T, st));
     StatLayout mlay{};
     bool mfused = false;
-    RUN(dgrad_with_bn_moments(net, t1, B.c3, B.c2, t3, &mlay, &mfused, st));
-    // ---- bn2 + conv2
-    RUN(conv_bn_backward(net, B.c2, t3, params, grads, t1, st, mfused ? &mlay : nullptr));
-    RUN(wgrad_step(net, B.c1.a, t1, B.c2, st));
-    RUN(dgrad_with_bn_moments(net, t1, B.c2, B.c1, t3, &mlay, &mfused, st));
-    // ---- bn1 + conv1
-    RUN(conv_bn_backward(net, B.c1, t3, params, grads, t1, st, mfused ? &mlay : nullptr));
+    RUN(dgrad_with_bn_moments(net, t1, T, M, t3, &mlay, &mfused, st));
+    // ---- M's BN (bottleneck: bn2, then conv2 and bn1; basic block: bn1)
+    RUN(conv_bn_backward(net, M, t3, params, grads, t1, st, mfused ? &mlay : nullptr));
+    if (!B.basic) {
+      RUN(wgrad_step(net, B.c1.a, t1, B.c2, st));
+      RUN(dgrad_with_bn_moments(net, t1, B.c2, B.c1, t3, &mlay, &mfused, st));
+      RUN(conv_bn_backward(net, B.c1, t3, params, grads, t1, st, mfused ? &mlay : nullptr));
+    }
+    // ---- conv1 (bn1 is done: t1 = the gradient of its output)
     RUN(wgrad_step(net, B.in, t1, B.c1, st));
     RUNP(kDgrad, conv_dgrad(t1, B.c1.wd, nA, B.c1.s, st));
     // ---- downsample branch
@@ -815,8 +852,8 @@ int dirb200_resnet_backward_blocks_stage(dirb200_net* net, int stage, const void
   net->bwd_blocks = true;
   const __nv_bfloat16* g3 = nullptr;
   if (stage > 0 && d_block) {
-    const Block& B = net->blocks[net->stage_begin[stage + 1] - 1];
-    const size_t bytes = sizeof(__nv_bfloat16) * (size_t)B.c3.rows * B.c3.s.cout;
+    const ConvLayer& T = net->blocks[net->stage_begin[stage + 1] - 1].tail();
+    const size_t bytes = sizeof(__nv_bfloat16) * (size_t)T.rows * T.s.cout;
     if (net->bwd_top < 0) {
       // the first gradient of this backward: it enters like the average-pool backward's output does
       net->bwd_top = stage;
@@ -867,7 +904,8 @@ extern "C" {
 /* Test / debugging aid: device pointer and shape of an internal activation.
  * block = -1: stem (which 0 = conv1 raw, 1 = relu(bn1), 6 = max-pool output, 7 = max-pool argmax);
  * block >= 0: which 0/1 = conv1 raw / act, 2/3 = conv2 raw / act, 4 = conv3 raw, 5 = downsample raw, 6 = block output,
- * 7 = the block output's ReLU mask.  Selectors 7 report bytes: *channels is the row length in bytes. */
+ * 7 = the block output's ReLU mask.  Selectors 7 report bytes: *channels is the row length in bytes.  A basic block
+ * has no conv3 (4 refused) and its conv2 is the tail: 3 is not materialised, 6 / 7 follow conv2. */
 int dirb200_resnet_peek(dirb200_net* net, int block, int which, void** ptr, int64_t* rows, int* channels) {
   // the selector is checked before the net is dereferenced
   DIRB_CHECK_ARG(which >= 0 && which <= 7, "resnet_peek: bad selector %d", which);
@@ -881,7 +919,7 @@ int dirb200_resnet_peek(dirb200_net* net, int block, int which, void** ptr, int6
     DIRB_CHECK_ARG(net->forward_was_training,
                    "resnet_peek: block ReLU mask not materialised (written by a training-mode forward only)");
     const Block& B = net->blocks[block];
-    *ptr = B.mask; *rows = B.c3.rows; *channels = B.c3.s.cout / 8;
+    *ptr = B.mask; *rows = B.tail().rows; *channels = B.tail().s.cout / 8;
     return DIRB200_OK;
   }
   if (block < 0) {
@@ -898,9 +936,9 @@ int dirb200_resnet_peek(dirb200_net* net, int block, int which, void** ptr, int6
       case 1: cv = &B.c1; act = true; break;
       case 2: cv = &B.c2; break;
       case 3: cv = &B.c2; act = true; break;
-      case 4: cv = &B.c3; break;
+      case 4: DIRB_CHECK_ARG(!B.basic, "resnet_peek: a basic block has no conv3"); cv = &B.c3; break;
       case 5: DIRB_CHECK_ARG(B.has_ds, "resnet_peek: block has no downsample"); cv = &B.ds; break;
-      case 6: *ptr = B.out; *rows = B.c3.rows; *channels = B.c3.s.cout; return DIRB200_OK;
+      case 6: *ptr = B.out; *rows = B.tail().rows; *channels = B.tail().s.cout; return DIRB200_OK;
       default: DIRB_CHECK_ARG(false, "resnet_peek: bad selector %d", which);
     }
   }
@@ -912,21 +950,23 @@ int dirb200_resnet_peek(dirb200_net* net, int block, int which, void** ptr, int6
 }
 
 /* Test / debugging aid: one conv layer's buffers, offset, shape and the split factor of its reduction-table entry.
- * block = -1: stem (conv 0); block >= 0: conv 0 / 1 / 2 / 3 = conv1 / conv2 / conv3 / downsample. */
+ * block = -1: stem (conv 0); block >= 0: conv 0 / 1 / 2 / 3 = conv1 / conv2 / conv3 / downsample (conv 2 refused for a
+ * basic block). */
 // The conv layer (block, conv) names and its entry in the split-K reduction table; `who` prefixes the refusals.
 static int find_conv(const dirb200_net* net, int block, int conv, const char* who, const ConvLayer** cv_out,
                      int* entry_out) {
   DIRB_CHECK_ARG(block >= -1 && block < (int)net->blocks.size(), "%s: bad block %d", who, block);
   DIRB_CHECK_ARG(conv >= 0 && conv <= (block < 0 ? 0 : 3), "%s: bad conv %d", who, conv);
-  // the reduction table holds the stem, then every block's c1, c2, c3 [, ds] in block order (build())
+  // the reduction table holds the stem, then every block's c1, c2 [, c3] [, ds] in block order (build())
   int entry = 0;
   const ConvLayer* cv = &net->stem;
   if (block >= 0) {
     const Block& B = net->blocks[block];
     DIRB_CHECK_ARG(conv < 3 || B.has_ds, "%s: block %d has no downsample", who, block);
+    DIRB_CHECK_ARG(conv != 2 || !B.basic, "%s: block %d is a basic block, it has no conv3", who, block);
     entry = 1;
-    for (int b = 0; b < block; ++b) entry += net->blocks[b].has_ds ? 4 : 3;
-    entry += conv;
+    for (int b = 0; b < block; ++b) entry += (net->blocks[b].basic ? 2 : 3) + (net->blocks[b].has_ds ? 1 : 0);
+    entry += conv == 3 && B.basic ? 2 : conv;
     const ConvLayer* convs[4] = {&B.c1, &B.c2, &B.c3, &B.ds};
     cv = convs[conv];
   }

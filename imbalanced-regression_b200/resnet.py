@@ -4,7 +4,10 @@
 attribute tree (conv1, bn1, layer1..4.{i}.{conv,bn}{1-3}, downsample.{0,1},
 linear, FDS), hence the reference's state_dict keys and shapes, the same
 `forward(x, targets=None, epoch=None)` contract (resnet.py:127-153) and the
-same initialisation (resnet.py:103-109).
+same initialisation (resnet.py:103-109).  `resnet18` / `resnet34` build the
+same over `BasicBlock` (resnet.py:14-38; conv1 / conv2 3x3, 512-d feature),
+`resnet101` / `resnet152` over deeper `Bottleneck` stacks
+(nyud2-dir/models/resnet.py:153-205).
 
 `E_resnet(resnet50())` is NYUD2-DIR's multi-scale encoder
 (nyud2-dir/models/modules.py:33-58): the same backbone without avgpool / fc,
@@ -34,6 +37,7 @@ print = logging.info
 P = c_void_p
 _lib.register({
     "dirb200_resnet_create": (c_int, [c_int, c_int, c_int, P, c_int, P]),
+    "dirb200_resnet_create_ex": (c_int, [c_int, c_int, c_int, c_int, P, c_int, P]),
     "dirb200_resnet_destroy": (None, [P]),
     "dirb200_resnet_param_count": (c_int64, [P]),
     "dirb200_resnet_running_count": (c_int64, [P]),
@@ -104,8 +108,23 @@ class _Linear(nn.Module):
         return _Linear1Fn.apply(x, self.weight, self.bias)
 
 
+class BasicBlock(nn.Module):
+    expansion = 1
+    kind = 1              # DIRB200_RESNET_BASIC
+
+    def __init__(self, inplanes, planes, stride=1, downsample=None):
+        super(BasicBlock, self).__init__()
+        self.conv1 = _Conv(inplanes, planes, 3, stride, 1)
+        self.bn1 = _BN(planes)
+        self.conv2 = _Conv(planes, planes, 3, 1, 1)
+        self.bn2 = _BN(planes)
+        self.downsample = downsample
+        self.stride = stride
+
+
 class Bottleneck(nn.Module):
     expansion = 4
+    kind = 0              # DIRB200_RESNET_BOTTLENECK
 
     def __init__(self, inplanes, planes, stride=1, downsample=None):
         super(Bottleneck, self).__init__()
@@ -196,7 +215,8 @@ class ResNet(nn.Module):
                  kernel='gaussian', ks=5, sigma=2, momentum=0.9, dropout=None):
         self.inplanes = 64
         super(ResNet, self).__init__()
-        assert block is Bottleneck, "the native runner implements the bottleneck ResNets (resnet50 and deeper)"
+        assert block in (BasicBlock, Bottleneck), "the native runner implements BasicBlock and Bottleneck ResNets"
+        self._block = block
         self._layers = list(layers)
         self.conv1 = _Conv(3, 64, 7, 2, 3)
         self.bn1 = _BN(64)
@@ -251,7 +271,9 @@ class ResNet(nn.Module):
         mods = [self.conv1, self.bn1]
         for layer in (self.layer1, self.layer2, self.layer3, self.layer4):
             for blk in layer:
-                mods += [blk.conv1, blk.bn1, blk.conv2, blk.bn2, blk.conv3, blk.bn3]
+                mods += [blk.conv1, blk.bn1, blk.conv2, blk.bn2]
+                if isinstance(blk, Bottleneck):
+                    mods += [blk.conv3, blk.bn3]
                 if blk.downsample is not None:
                     mods += [blk.downsample[0], blk.downsample[1]]
         return mods
@@ -347,7 +369,7 @@ class ResNet(nn.Module):
             assert c == 3, "expected NCHW input with 3 channels"
             handle = c_void_p()
             arr = (c_int * 4)(*self._layers)
-            _lib.call("dirb200_resnet_create", n, h, w, arr, 4, ctypes.byref(handle))
+            _lib.call("dirb200_resnet_create_ex", n, h, w, self._block.kind, arr, 4, ctypes.byref(handle))
             assert _lib.raw("dirb200_resnet_param_count")(handle) == self._flat["backbone"], "parameter layout mismatch"
             assert _lib.raw("dirb200_resnet_running_count")(handle) == self._flat["running"].numel()
             net = handle
@@ -369,7 +391,7 @@ class ResNet(nn.Module):
         _lib.require_cuda(x, self._flat["params"])
         x = x.detach().to(torch.float32).contiguous()
         net = self._net(tuple(x.shape))
-        enc = torch.empty(x.shape[0], 512 * Bottleneck.expansion, dtype=torch.float32, device=x.device)
+        enc = torch.empty(x.shape[0], 512 * self._block.expansion, dtype=torch.float32, device=x.device)
         _lib.call("dirb200_resnet_forward", net, _lib.ptr(x), _lib.ptr(self._flat["params"]),
                   _lib.ptr(self._flat["running"]), int(training), _lib.ptr(enc), _lib.stream_ptr())
         if training:
@@ -377,13 +399,13 @@ class ResNet(nn.Module):
         return enc
 
     def _run_forward_blocks(self, x, training):
-        """x fp32 NCHW [n, 3, h, w] -> the outputs of layer1..4, NHWC bf16 [n, h_s, w_s, 256 << s]."""
+        """x fp32 NCHW [n, 3, h, w] -> the outputs of layer1..4, NHWC bf16 [n, h_s, w_s, (64 << s) * expansion]."""
         _lib.require_cuda(x, self._flat["params"])
         x = x.detach().to(torch.float32).contiguous()
         n, _, h, w = x.shape
         net = self._net(tuple(x.shape))
         maps = _feature_maps(h, w, len(self._layers))[1:]
-        outs = [torch.empty(n, hs, ws, 64 * Bottleneck.expansion << s, dtype=torch.bfloat16, device=x.device)
+        outs = [torch.empty(n, hs, ws, 64 * self._block.expansion << s, dtype=torch.bfloat16, device=x.device)
                 for s, (hs, ws) in enumerate(maps)]
         ptrs = (c_void_p * len(outs))(*[o.data_ptr() for o in outs])
         _lib.call("dirb200_resnet_forward_blocks", net, _lib.ptr(x), _lib.ptr(self._flat["params"]),
@@ -486,17 +508,35 @@ class ResNet(nn.Module):
             return x
 
 
+def resnet18(**kwargs):
+    return ResNet(BasicBlock, [2, 2, 2, 2], **kwargs)
+
+
+def resnet34(**kwargs):
+    return ResNet(BasicBlock, [3, 4, 6, 3], **kwargs)
+
+
 def resnet50(**kwargs):
     return ResNet(Bottleneck, [3, 4, 6, 3], **kwargs)
+
+
+def resnet101(**kwargs):
+    return ResNet(Bottleneck, [3, 4, 23, 3], **kwargs)
+
+
+def resnet152(**kwargs):
+    return ResNet(Bottleneck, [3, 8, 36, 3], **kwargs)
 
 
 class E_resnet(nn.Module):
     """NYUD2-DIR's encoder (nyud2-dir/models/modules.py:33-58): `original_model`'s stem and layer1..4 without avgpool /
     linear.  It shares the native ResNet's holders, flat parameter / gradient / running-statistics buffers and runner
-    cache, so its state_dict has the reference E_resnet's keys and loads a torchvision-layout ResNet-50 checkpoint.
+    cache, so its state_dict has the reference E_resnet's keys and loads a torchvision-layout checkpoint of the same
+    depth (resnet18 ... resnet152).
 
     forward(x): x fp32 NCHW [B, 3, H, W] (H, W multiples of 4) -> (x_block1, x_block2, x_block3, x_block4), NHWC bf16
-    [B, h_s, w_s, C_s] with C_s = 256, 512, 1024, 2048 (the layout dense_ops consumes).  In training mode with
+    [B, h_s, w_s, C_s] with C_s = 256, 512, 1024, 2048 over Bottleneck (resnet50 / 101 / 152) and 64, 128, 256, 512 over
+    BasicBlock (resnet18 / 34) (the layout dense_ops consumes).  In training mode with
     gradients enabled they carry autograd history into the backbone parameters; x receives no gradient."""
 
     def __init__(self, original_model, num_features=2048):

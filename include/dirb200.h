@@ -529,25 +529,35 @@ int dirb200_bn_eval_coeffs_all(const dirb200_bn_eval_job* jobs_host, int njobs, 
                                const float* running, float eps, void* stream);
 
 /* ------------------------------------------------ ResNet backbone runner ---- */
-/* Opaque native runner of the bottleneck ResNet of agedb-dir/resnet.py:41-70,
- * 73-138 (conv1/bn1/relu/maxpool, layer1-4, avgpool, view) for one fixed
- * input shape.  It owns every activation / gradient / operand buffer (NHWC
- * bf16); parameters, their gradients and the BN running statistics stay in
- * caller-owned flat fp32 buffers laid out in the reference's
- * named_parameters() order: conv1.weight, bn1.weight, bn1.bias, then per
- * block conv1.weight, bn1.{weight,bias}, conv2.weight, bn2.*, conv3.weight,
- * bn3.*, [downsample.0.weight, downsample.1.{weight,bias}]; running stats per
- * BN in the same order as (running_mean, running_var). */
+/* Opaque native runner of the ResNet of agedb-dir/resnet.py:14-38 (BasicBlock)
+ * or 41-70 (Bottleneck), 73-138 (conv1/bn1/relu/maxpool, layer1-4, avgpool,
+ * view) for one fixed input shape.  It owns every activation / gradient /
+ * operand buffer (NHWC bf16); parameters, their gradients and the BN running
+ * statistics stay in caller-owned flat fp32 buffers laid out in the
+ * reference's named_parameters() order: conv1.weight, bn1.weight, bn1.bias,
+ * then per block conv1.weight, bn1.{weight,bias}, conv2.weight, bn2.*,
+ * [conv3.weight, bn3.* (bottleneck only)], [downsample.0.weight,
+ * downsample.1.{weight,bias}]; running stats per BN in the same order as
+ * (running_mean, running_var). */
 typedef struct dirb200_net dirb200_net;
+
+/* Block kinds of dirb200_resnet_create_ex.  Bottleneck: conv1 1x1, conv2 3x3 with the stride, conv3 1x1 to 4 x planes
+ * (ResNet-50 / 101 / 152).  Basic: conv1 3x3 with the stride, conv2 3x3 (ResNet-18 / 34; 512-d feature). */
+#define DIRB200_RESNET_BOTTLENECK 0
+#define DIRB200_RESNET_BASIC 1
 
 /* H and W: multiples of 4 (the input space-to-depth needs even H, W; the max-pool backward an even stem output), at
  * most 1024 (the convolutions pack a stem-output row / column in 9 bits); N at most 8192 (13 bits of image index),
  * and N * H/2 * W/2 < 2^31. */
 int dirb200_resnet_create(int n, int h, int w, const int* blocks_per_stage, int num_stages, dirb200_net** out);
+/* The same with the block kind (DIRB200_RESNET_*); dirb200_resnet_create is block = DIRB200_RESNET_BOTTLENECK.  Any
+ * other block value is refused before a CUDA call. */
+int dirb200_resnet_create_ex(int n, int h, int w, int block, const int* blocks_per_stage, int num_stages,
+                             dirb200_net** out);
 void dirb200_resnet_destroy(dirb200_net* net);
 int64_t dirb200_resnet_param_count(const dirb200_net* net);   /* floats in the flat parameter buffer */
 int64_t dirb200_resnet_running_count(const dirb200_net* net); /* floats in the flat BN running buffer */
-int64_t dirb200_resnet_feature_dim(const dirb200_net* net);   /* 2048 for ResNet-50 */
+int64_t dirb200_resnet_feature_dim(const dirb200_net* net);   /* 2048 for ResNet-50 and deeper, 512 for ResNet-18 / 34 */
 int64_t dirb200_resnet_device_bytes(const dirb200_net* net);
 
 /* ResNet.forward up to `encoding` (resnet.py:128-138): x fp32 NCHW -> enc fp32
@@ -570,8 +580,9 @@ int dirb200_resnet_stage_param_range(const dirb200_net* net, int stage, int64_t*
 
 /* Multi-scale encoder forward (nyud2-dir/models/modules.py:33-58, E_resnet.forward): the forward above without the
  * average pool; block_out[s] receives the output of the last block of layer group s+1 as NHWC bf16 [n, h_s, w_s, C_s]
- * (256 / 512 / 1024 / 2048 channels for ResNet-50).  training == 0: running statistics (folded-BN forward).  Every layer
- * group must end in an identity block (true of ResNet-50 and deeper). */
+ * (256 / 512 / 1024 / 2048 channels for a bottleneck net, 64 / 128 / 256 / 512 for a basic-block one).  training == 0:
+ * running statistics (folded-BN forward).  Every layer group must end in an identity block (true of ResNet-18 and
+ * deeper). */
 int dirb200_resnet_forward_blocks(dirb200_net* net, const float* x_nchw, const float* params, float* bn_running,
                                   int training, void* const* block_out, void* stream);
 
@@ -595,11 +606,12 @@ int dirb200_resnet_read_profile(dirb200_net* net, double* ms_by_kind, int64_t* g
  * the window's first maximum); block >= 0: 0/1 = conv1 raw / act, 2/3 = conv2 raw / act, 4 = conv3 raw,
  * 5 = downsample raw, 6 = block output, 7 = the block output's ReLU mask: [rows][channels] bytes with
  * channels = C / 8, bit j of byte g = (output channel 8g + j > 0); refused unless the last forward was a training one.
+ * A basic block's conv2 is its tail: 6 / 7 follow it, 3 is not materialised and 4 (conv3) is refused.
  * A selector outside 0 .. 7, or 2 .. 5 for the stem, is refused before net is read. */
 int dirb200_resnet_peek(dirb200_net* net, int block, int which, void** ptr, int64_t* rows, int* channels);
 
 /* Test / debugging aid: one conv layer's own buffers and descriptor entries.  block = -1: the stem (conv 0);
- * block >= 0: conv 0 / 1 / 2 / 3 = conv1 / conv2 / conv3 / downsample.  w_fprop / w_dgrad: its bf16 GEMM operands
+ * block >= 0: conv 0 / 1 / 2 / 3 = conv1 / conv2 / conv3 / downsample (conv 2 refused for a basic block).  w_fprop / w_dgrad: its bf16 GEMM operands
  * (w_dgrad NULL for the stem); partial: its split-K weight-gradient partials [splits][cout][kh*kw*cin] (stem:
  * [splits][cout][256]); scale / shift: its BatchNorm's fp32 [cout] coefficients; w_off: its weight's offset in the flat
  * parameter buffer; cout .. pad: the conv's hyper-parameters (stem: 3 -> cout, 7x7, stride 2, pad 3); splits: the

@@ -52,6 +52,10 @@ struct Block {
 
 using namespace dirb200;
 
+// backward-tap selectors (dirb200_resnet_peek_backward, include/dirb200.h)
+enum TapSel { kTapGA = 0, kTapGB, kTapG3, kTapDz, kTapDyTail, kTapDyDs, kTapDgradTail, kTapDyPreTail, kTapDgradC2,
+              kTapDyC1, kTapNA, kTapNB, kTapPool, kTapDyStem, kNumTaps };
+
 struct dirb200_net {
   int n = 0, h = 0, w = 0;
   int block = DIRB200_RESNET_BOTTLENECK;
@@ -104,6 +108,13 @@ struct dirb200_net {
   struct ProfRec { int kind; cudaEvent_t a, b; };
   std::vector<ProfRec> prof;
   std::vector<cudaEvent_t> event_pool;
+  // backward tap (dirb200_resnet_set_backward_tap): copies of the transient gradients of one block (or the stem)
+  int tap_block = DIRB200_RESNET_NO_TAP;
+  __nv_bfloat16* tap[kNumTaps] = {};   // each holds max_act elements; allocated by the first set call
+  size_t max_act = 0;
+  int64_t tap_rows[kNumTaps] = {};
+  int tap_ch[kNumTaps] = {};
+  unsigned tap_written = 0;            // bit s: selector s was written by the last backward
 };
 
 namespace dirb200 {
@@ -212,6 +223,7 @@ static bool build(dirb200_net* net, const int* blocks_per_stage, int num_stages)
   net->stage_begin.push_back((int)net->blocks.size());
   net->feat_c = inplanes;
   net->feat_hw = h * w;
+  net->max_act = max_act;
   for (int i = 0; i < 8; ++i) NET_ALLOC(net->scratch[i], max_act * 2);
   {
     // split-K reduction jobs: every conv owns its partial buffer; one launch reduces a whole backward stage
@@ -684,6 +696,20 @@ int dirb200_resnet_forward_blocks(dirb200_net* net, const float* x_nchw, const f
 
 namespace dirb200 {
 
+// Backward tap: when `block` (-1: the stem) is the tapped one, a copy of p ([rows][ch] bf16) goes into tap buffer
+// `which`, on the launch stream right after the launch that produced it.  With no tap set nothing is issued: the launch
+// sequence of a training step is unchanged.
+static int tap_copy(dirb200_net* net, int block, int which, const __nv_bfloat16* p, int64_t rows, int ch,
+                    cudaStream_t st) {
+  if (net->tap_block != block || p == nullptr) return DIRB200_OK;
+  DIRB_CUDA(cudaMemcpyAsync(net->tap[which], p, sizeof(__nv_bfloat16) * (size_t)rows * ch, cudaMemcpyDeviceToDevice,
+                            st));
+  net->tap_rows[which] = rows;
+  net->tap_ch[which] = ch;
+  net->tap_written |= 1u << which;
+  return DIRB200_OK;
+}
+
 // blocks [lo, hi) in reverse order; the incoming gradient pair is net->bw_gA / bw_gB, plus g3 (may be null) for the
 // output of block hi-1 (multi-scale mode: the gradient of a layer group's output from outside the network)
 static int backward_blocks(dirb200_net* net, int lo, int hi, const float* params, float* grads, cudaStream_t st,
@@ -699,11 +725,16 @@ static int backward_blocks(dirb200_net* net, int lo, int hi, const float* params
     // ---- block output: out = relu(bn_T(y_T) + identity); dz = (gA + gB) * (out > 0)
     int nblk = 0;
     const int kparts = B.has_ds ? 3 : 2;
+    const int n = T.s.n;
+    RUN(tap_copy(net, bi, kTapGA, gA, T.rows, b3.c, st));
+    RUN(tap_copy(net, bi, kTapGB, gB, gB_h ? (int64_t)n * (gB_h / 2) * (gB_w / 2) : T.rows, b3.c, st));
+    if (bi == hi - 1) RUN(tap_copy(net, bi, kTapG3, g3, T.rows, b3.c, st));
     // identity blocks: the reduction also stores dz (= the gradient of the shortcut path, nB) so that the apply pass
     // reads ONE gradient tensor instead of gA, gB and the mask again
     RUNP(kBnBwdReduce, bn_bwd_reduce(gA, gB, T.y, B.has_ds ? B.ds.y : nullptr, nullptr, nullptr, B.mask, T.rows,
                                      b3.c, net->bn_partial, &nblk, st, gB_h, gB_w, B.has_ds ? nullptr : nB,
                                      bi == hi - 1 ? g3 : nullptr));
+    if (!B.has_ds) RUN(tap_copy(net, bi, kTapDz, nB, T.rows, b3.c, st));
     if (B.has_ds) {
       BNLayer& bd = B.ds.bn;
       RUNP(kBnBwdApply, bn_bwd_coeffs(net->bn_partial, nblk, kparts, 2, T.rows, b3.c, bd.mean, bd.invstd,
@@ -717,22 +748,29 @@ static int backward_blocks(dirb200_net* net, int lo, int hi, const float* params
     else
       RUNP(kBnBwdApply, bn_bwd_apply(nB, nullptr, T.y, b3.coef, nullptr, nullptr, nullptr, nullptr, nullptr, T.rows,
                                      b3.c, t1, nullptr, nullptr, st));
+    RUN(tap_copy(net, bi, kTapDyTail, t1, T.rows, b3.c, st));
+    if (B.has_ds) RUN(tap_copy(net, bi, kTapDyDs, t2, T.rows, b3.c, st));
     gB_h = gB_w = 0;
     // ---- tail conv
     RUN(wgrad_step(net, M.a, t1, T, st));
     StatLayout mlay{};
     bool mfused = false;
     RUN(dgrad_with_bn_moments(net, t1, T, M, t3, &mlay, &mfused, st));
+    RUN(tap_copy(net, bi, kTapDgradTail, t3, M.rows, M.s.cout, st));
     // ---- M's BN (bottleneck: bn2, then conv2 and bn1; basic block: bn1)
     RUN(conv_bn_backward(net, M, t3, params, grads, t1, st, mfused ? &mlay : nullptr));
+    RUN(tap_copy(net, bi, kTapDyPreTail, t1, M.rows, M.s.cout, st));
     if (!B.basic) {
       RUN(wgrad_step(net, B.c1.a, t1, B.c2, st));
       RUN(dgrad_with_bn_moments(net, t1, B.c2, B.c1, t3, &mlay, &mfused, st));
+      RUN(tap_copy(net, bi, kTapDgradC2, t3, B.c1.rows, B.c1.s.cout, st));
       RUN(conv_bn_backward(net, B.c1, t3, params, grads, t1, st, mfused ? &mlay : nullptr));
+      RUN(tap_copy(net, bi, kTapDyC1, t1, B.c1.rows, B.c1.s.cout, st));
     }
     // ---- conv1 (bn1 is done: t1 = the gradient of its output)
     RUN(wgrad_step(net, B.in, t1, B.c1, st));
     RUNP(kDgrad, conv_dgrad(t1, B.c1.wd, nA, B.c1.s, st));
+    RUN(tap_copy(net, bi, kTapNA, nA, (int64_t)n * B.c1.s.h * B.c1.s.w, B.c1.s.cin, st));
     // ---- downsample branch
     if (B.has_ds) {
       RUN(wgrad_step(net, B.in, t2, B.ds, st));
@@ -744,10 +782,12 @@ static int backward_blocks(dirb200_net* net, int lo, int hi, const float* params
         // the even positions (no memset of the full map, no scattered store, no dense re-reads of zeros)
         const ConvShape cs{d.n, d.ho, d.wo, d.cin, d.cout, 1, 1, 1, 0, d.ho, d.wo};
         RUNP(kDgrad, conv_dgrad(t2, B.ds.wd, nB, cs, st));
+        RUN(tap_copy(net, bi, kTapNB, nB, (int64_t)n * d.ho * d.wo, d.cin, st));
         gB_h = d.h;
         gB_w = d.w;
       } else {
         RUNP(kDgrad, conv_dgrad(t2, B.ds.wd, nB, B.ds.s, st));
+        RUN(tap_copy(net, bi, kTapNB, nB, (int64_t)n * d.h * d.w, d.cin, st));
       }
     }
     // the two gradients w.r.t. this block's input become the next (earlier) block's incoming pair
@@ -773,14 +813,20 @@ static int backward_stage_run(dirb200_net* net, int stage, const float* params, 
     } else {
       // ---- stem: maxpool -> bn1+relu -> conv1 (no data gradient needed)
       __nv_bfloat16 *t1 = net->scratch[4], *t3 = net->scratch[6];
+      const int64_t pool_rows = (int64_t)net->n * net->pool_h * net->pool_w;
+      RUN(tap_copy(net, -1, kTapGA, net->bw_gA, pool_rows, 64, st));
+      RUN(tap_copy(net, -1, kTapGB, net->bw_gB, pool_rows, 64, st));
       RUNP(kPool, maxpool_bwd(net->bw_gA, net->bw_gB, net->pool_idx, net->n, net->stem.s.ho, net->stem.s.wo, 64, t3, st));
+      RUN(tap_copy(net, -1, kTapPool, t3, net->stem.rows, 64, st));
       RUN(conv_bn_backward(net, net->stem, t3, params, grads, t1, st));
+      RUN(tap_copy(net, -1, kTapDyStem, t1, net->stem.rows, 64, st));
       RUN(wgrad_step(net, net->x_s2d, t1, net->stem, st));
     }
     RUN(wgrad_reduce_stage(net, stage, grads, st));
     return DIRB200_OK;
   };
-  if (!graphs_enabled() || net->profiling) return body(st);
+  // a tapped backward runs eagerly (the copies are not part of the captured sequence); the slot is left as it was
+  if (!graphs_enabled() || net->profiling || net->tap_block != DIRB200_RESNET_NO_TAP) return body(st);
   const bool replay = g.exec && g.k0 == params && g.k1 == grads;
   RUN(run_graphed(net, g, params, grads, st, body));
   if (replay) {
@@ -812,6 +858,7 @@ int dirb200_resnet_backward_stage(dirb200_net* net, int stage, const float* d_en
   if (stage == nst) {
     DIRB_CHECK_ARG(net->forward_was_training, "resnet_backward: needs a preceding training-mode forward");
     DIRB_CHECK_ARG(d_enc, "resnet_backward_stage: the first stage needs d_enc");
+    net->tap_written = 0;
     net->bw_gA = net->scratch[0]; net->bw_gB = nullptr; net->bw_nA = net->scratch[2]; net->bw_nB = net->scratch[3];
     net->bw_spareB = net->scratch[1];
     net->bw_gB_h = net->bw_gB_w = 0;
@@ -843,6 +890,7 @@ int dirb200_resnet_backward_blocks_stage(dirb200_net* net, int stage, const void
   if (stage == nst) {
     DIRB_CHECK_ARG(net->forward_was_training, "resnet_backward_blocks_stage: needs a preceding training-mode forward");
     net->bwd_top = -1;
+    net->tap_written = 0;
   } else {
     DIRB_CHECK_ARG(net->bwd_next_stage == stage && net->bwd_blocks,
                    "resnet_backward_blocks_stage: stage %d out of order (expected %d%s)", stage, net->bwd_next_stage,
@@ -1010,6 +1058,49 @@ int dirb200_resnet_peek_bn_stats(dirb200_net* net, int block, int conv, float** 
   RUN(find_conv(net, block, conv, "resnet_peek_bn_stats", &cv, &entry));
   *mean = cv->bn.mean;
   *invstd = cv->bn.invstd;
+  return DIRB200_OK;
+}
+
+/* Test / debugging aid: one conv's BatchNorm-backward coefficients, fp32 [3][cout] (A, B, C of dy = A dz + B y + C),
+ * as the last backward left them.  block / conv as dirb200_resnet_peek_conv. */
+int dirb200_resnet_peek_bn_coef(dirb200_net* net, int block, int conv, float** coef) {
+  DIRB_CHECK_ARG(net && coef, "resnet_peek_bn_coef: null pointer");
+  int entry = 0;
+  const ConvLayer* cv = nullptr;
+  RUN(find_conv(net, block, conv, "resnet_peek_bn_coef", &cv, &entry));
+  *coef = cv->bn.coef;
+  return DIRB200_OK;
+}
+
+int dirb200_resnet_set_backward_tap(dirb200_net* net, int block) {
+  DIRB_CHECK_ARG(block >= DIRB200_RESNET_NO_TAP, "resnet_set_backward_tap: bad block %d", block);
+  DIRB_CHECK_ARG(net, "resnet_set_backward_tap: null net");
+  DIRB_CHECK_ARG(block < (int)net->blocks.size(), "resnet_set_backward_tap: bad block %d", block);
+  if (block != DIRB200_RESNET_NO_TAP && !net->tap[0]) {
+    for (auto& t : net->tap) {
+      DIRB_CUDA(cudaMalloc(&t, net->max_act * sizeof(__nv_bfloat16)));
+      net->allocs.push_back(t);
+    }
+  }
+  net->tap_block = block;
+  return DIRB200_OK;
+}
+
+static const char* const kTapNames[kNumTaps] = {"gA", "gB", "g3", "dz", "tail dy", "downsample dy", "tail dgrad",
+                                               "pre-tail dy", "conv2 dgrad", "conv1 dy", "nA", "nB",
+                                               "max-pool backward", "stem dy"};
+
+int dirb200_resnet_peek_backward(dirb200_net* net, int which, void** ptr, int64_t* rows, int* channels) {
+  // the selector is checked before the net is read
+  DIRB_CHECK_ARG(which >= 0 && which < kNumTaps, "resnet_peek_backward: bad selector %d", which);
+  DIRB_CHECK_ARG(net && ptr && rows && channels, "resnet_peek_backward: null pointer");
+  DIRB_CHECK_ARG(net->tap_block != DIRB200_RESNET_NO_TAP, "resnet_peek_backward: no backward tap is set");
+  DIRB_CHECK_ARG((net->tap_written >> which) & 1u,
+                 "resnet_peek_backward: selector %d (%s) was not written by the last backward of block %d", which,
+                 kTapNames[which], net->tap_block);
+  *ptr = net->tap[which];
+  *rows = net->tap_rows[which];
+  *channels = net->tap_ch[which];
   return DIRB200_OK;
 }
 }

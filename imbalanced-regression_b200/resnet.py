@@ -53,6 +53,9 @@ _lib.register({
     "dirb200_resnet_peek": (c_int, [P, c_int, c_int, P, P, P]),
     "dirb200_resnet_peek_conv": (c_int, [P, c_int, c_int, P]),
     "dirb200_resnet_peek_bn_stats": (c_int, [P, c_int, c_int, P, P]),
+    "dirb200_resnet_peek_bn_coef": (c_int, [P, c_int, c_int, P]),
+    "dirb200_resnet_set_backward_tap": (c_int, [P, c_int]),
+    "dirb200_resnet_peek_backward": (c_int, [P, c_int, P, P, P]),
     "dirb200_resnet_forward_blocks": (c_int, [P, P, P, P, c_int, P, P]),
     "dirb200_resnet_backward_blocks_stage": (c_int, [P, c_int, P, P, P, P]),
     "dirb200_linear1_fwd": (c_int, [P, P, P, c_int64, c_int, P, P]),

@@ -631,6 +631,29 @@ int dirb200_resnet_peek_conv(dirb200_net* net, int block, int conv, dirb200_conv
  * training-mode forward left them (its own entry point: dirb200_conv_peek keeps its layout, which callers allocate). */
 int dirb200_resnet_peek_bn_stats(dirb200_net* net, int block, int conv, float** mean, float** invstd);
 
+/* Test / debugging aid: the same conv's BatchNorm-backward coefficients, fp32 [3][cout] (A, B, C of
+ * dy = A dz + B y + C), as the last backward left them. */
+int dirb200_resnet_peek_bn_coef(dirb200_net* net, int block, int conv, float** coef);
+
+/* Test / debugging aid: the backward tap.  While block b is tapped (-1: the stem, 0 .. blocks-1), every backward copies
+ * the transient gradients of that block, each right after the launch that produces it, into buffers the net owns
+ * (allocated by the first call that sets a tap, freed with the net), and runs its stages eagerly (no CUDA graph capture
+ * or replay).  DIRB200_RESNET_NO_TAP switches the tap off: the backward is then exactly the untapped one.
+ * dirb200_resnet_peek_backward returns one tapped tensor of the last backward, [rows][channels] bf16 NHWC:
+ *   0 / 1  incoming gA / gB of the block (gB: the compact [n, h/2, w/2, c] gradient of the next block's stride-2 1x1
+ *          downsample where that form is taken, rows as such); the stem's: the gradients of the max-pool output
+ *   2      g3, the multi-scale gradient of the block output (last block of a layer group)
+ *   3      dz = mask (gA + gB [+ g3]) as the block-output reduction stored it (identity blocks)
+ *   4 / 5  dy of the tail conv (bottleneck conv3, basic conv2) / of the downsample, after the BN backward
+ *   6 / 7  tail-conv dgrad output / dy of the pre-tail conv (conv2 / conv1) after its BN backward
+ *   8 / 9  bottleneck only: conv2 dgrad output / dy of conv1
+ *   10/11  conv1 dgrad output nA / downsample dgrad output nB (compact as for 1, or the full map)
+ *   12/13  stem only: max-pool backward output / dy of the stem conv
+ * A selector outside 0 .. 13 is refused before net is read; one the last backward did not write is refused. */
+#define DIRB200_RESNET_NO_TAP (-2)
+int dirb200_resnet_set_backward_tap(dirb200_net* net, int block);
+int dirb200_resnet_peek_backward(dirb200_net* net, int which, void** ptr, int64_t* rows, int* channels);
+
 /* nn.Linear(feature_dim, 1) (resnet.py:88,148): pred[n] = x[n,d] . w[d] + bias */
 int dirb200_linear1_fwd(const float* x, const float* w, const float* bias, int64_t n, int d, float* pred,
                         void* stream);

@@ -453,6 +453,27 @@ def run_pool_fwd(shape, seed, img_chunk=16):
     return idx
 
 
+def maxpool_bwd_ref(g1, g2, idx, h, w):
+    """float64 max-pool backward of g1 [+ g2] ([n, ho, wo, c] bf16) through the argmax idx onto the h x w map, flat NHWC:
+    (ref, the bound 2^-8 |ref| + 4 u sum |g| of the kernel's fp32 sums and one bf16 rounding, windows per pixel)."""
+    n, ho, wo, c = idx.shape
+    yo = torch.arange(ho, device=DEV).view(1, ho, 1, 1)
+    xo = torch.arange(wo, device=DEV).view(1, 1, wo, 1)
+    ch = torch.arange(c, device=DEV).view(1, 1, 1, c)
+    k = idx.long()
+    iy, ix = 2 * yo - 1 + k // 3, 2 * xo - 1 + k % 3
+    assert ((iy >= 0) & (iy < h) & (ix >= 0) & (ix < w)).all()
+    im = torch.arange(n, device=DEV).view(n, 1, 1, 1)
+    flat = (((im * h + iy) * w + ix) * c + ch).reshape(-1)
+    gv = g1.double() + (g2.double() if g2 is not None else 0.0)
+    ga = g1.double().abs() + (g2.double().abs() if g2 is not None else 0.0)
+    size = n * h * w * c
+    ref = torch.zeros(size, dtype=F64, device=DEV).index_add_(0, flat, gv.reshape(-1))
+    mag = torch.zeros(size, dtype=F64, device=DEV).index_add_(0, flat, ga.reshape(-1))
+    cnt = torch.zeros(size, dtype=torch.int32, device=DEV).index_add_(0, flat, torch.ones_like(flat, dtype=torch.int32))
+    return ref, 2.0 ** -8 * ref.abs() + 4 * U * mag, cnt
+
+
 def check_pool_bwd(shape, idx, seed, with_g2, img_chunk=16):
     L = lib()
     n, h, w, c = shape
@@ -463,29 +484,15 @@ def check_pool_bwd(shape, idx, seed, with_g2, img_chunk=16):
     dx = torch.full((n, h, w, c), float("nan"), dtype=BF, device=DEV)
     L.call("dirb200_layer_maxpool_bwd", L.ptr(g1), L.ptr(g2), L.ptr(idx), n, h, w, c, L.ptr(dx), L.stream_ptr())
     torch.cuda.synchronize()
-    yo = torch.arange(ho, device=DEV).view(1, ho, 1, 1)
-    xo = torch.arange(wo, device=DEV).view(1, 1, wo, 1)
-    ch = torch.arange(c, device=DEV).view(1, 1, 1, c)
     multi = 0
     for b0 in range(0, n, img_chunk):
         b = slice(b0, min(n, b0 + img_chunk))
-        nb = b.stop - b.start
-        k = idx[b].long()
-        iy, ix = 2 * yo - 1 + k // 3, 2 * xo - 1 + k % 3
-        assert ((iy >= 0) & (iy < h) & (ix >= 0) & (ix < w)).all()
-        im = torch.arange(nb, device=DEV).view(nb, 1, 1, 1)
-        flat = (((im * h + iy) * w + ix) * c + ch).reshape(-1)
-        gv = g1[b].double() + (g2[b].double() if with_g2 else 0.0)
-        ga = g1[b].double().abs() + (g2[b].double().abs() if with_g2 else 0.0)
-        size = nb * h * w * c
-        ref = torch.zeros(size, dtype=F64, device=DEV).index_add_(0, flat, gv.reshape(-1))
-        mag = torch.zeros(size, dtype=F64, device=DEV).index_add_(0, flat, ga.reshape(-1))
-        cnt = torch.zeros(size, dtype=torch.int32, device=DEV).index_add_(0, flat, torch.ones_like(flat, dtype=torch.int32))
+        ref, bound, cnt = maxpool_bwd_ref(g1[b], g2[b] if with_g2 else None, idx[b], h, w)
         got = dx[b].reshape(-1)
         zero = cnt == 0
         assert (bits(got)[zero] == 0).all(), "a pixel that is no window's argmax is not exactly 0"
         e = (got.double() - ref).abs()
-        ok = e <= 2.0 ** -8 * ref.abs() + 4 * U * mag
+        ok = e <= bound
         assert ok.all(), f"maxpool_bwd (g2={with_g2}): {int((~ok).sum())} pixels outside the bound"
         multi += int((cnt > 1).sum())
     if ho * wo >= 4:

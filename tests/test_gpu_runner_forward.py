@@ -37,6 +37,7 @@ Every training case runs three forwards on fresh inputs and parameters: eager, t
 a replay (run_graphed, csrc/resnet_runner.cu).  Each must pass every check.  The whole file runs again in subprocesses
 with DIRB200_SMS=7, DIRB200_GRAPH=0 and DIRB200_FUSED_STATS=0."""
 import ctypes
+import gc
 import os
 import subprocess
 import sys
@@ -532,15 +533,22 @@ def test_eval_forward_in_place(layers, n, h, w, blocks):
 
 
 # ------------------------------------------------------------------------------------------------ reruns
-def rerun(env, *select):
+def rerun(env, *select, path=os.path.abspath(__file__)):
+    """pytest on `path` (this file) in a fresh process with `env` added; prints its "worst" lines.  This process first
+    hands its cached device memory back, so that the child has the card's memory; a failure's message starts with the
+    child's own failure lines."""
+    gc.collect()
+    torch.cuda.empty_cache()
     e = dict(os.environ)
     e.update(env)
     t0 = time.time()
     r = subprocess.run([sys.executable, "-m", "pytest", "-q", "-x", "-s", "-p", "no:cacheprovider",
-                        os.path.abspath(__file__), *select], env=e, cwd=ROOT, capture_output=True, text=True,
+                        path, *select], env=e, cwd=ROOT, capture_output=True, text=True,
                        timeout=3000)
     print(f"\n{env}: {time.time() - t0:.1f} s\n" + "\n".join(l for l in r.stdout.splitlines() if "worst" in l)[-3000:])
-    assert r.returncode == 0, r.stdout[-4000:] + r.stderr[-2000:]
+    why = [l for l in (r.stdout + r.stderr).splitlines() if l.startswith(("FAILED", "ERROR", "E "))]
+    assert r.returncode == 0, (f"{env}: rc {r.returncode}: " + " | ".join(why[:6])[:1500] + "\n" + r.stdout[-4000:] +
+                               r.stderr[-2000:])
 
 
 RERUN_VARS = ("DIRB200_SMS", "DIRB200_GRAPH", "DIRB200_FUSED_STATS", "DIRB200_FOLDED_EVAL")

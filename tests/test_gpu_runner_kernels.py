@@ -363,31 +363,36 @@ def test_bn_eval_coeffs_all_against_float64():
 
 
 # ------------------------------------------------------------------------------------------------ in place
-def conv_table(layers, H, W):
+def conv_table(layers, H, W, basic=False):
     """Every conv of the runner in its build order: (block, conv, weight name, BN prefix, cin, cout, k, stride, pad,
-    input h, input w, stem)."""
+    input h, input w, stem).  basic: BasicBlock nets (conv1 3x3 with the stride, conv2 3x3; no conv 2)."""
     out = [(-1, 0, "conv1.weight", "bn1.", 3, 64, 7, 2, 3, H, W, 1)]
     h, w = (H // 2 - 1) // 2 + 1, (W // 2 - 1) // 2 + 1
     inpl, bi = 64, 0
     for li, nb in enumerate(layers):
         pl = 64 << li
+        outc = pl if basic else pl * 4
         for b in range(nb):
             s = 2 if (b == 0 and li > 0) else 1
             pre = f"layer{li + 1}.{b}."
             ho, wo = (h - 1) // s + 1, (w - 1) // s + 1
-            out += [(bi, 0, pre + "conv1.weight", pre + "bn1.", inpl, pl, 1, 1, 0, h, w, 0),
-                    (bi, 1, pre + "conv2.weight", pre + "bn2.", pl, pl, 3, s, 1, h, w, 0),
-                    (bi, 2, pre + "conv3.weight", pre + "bn3.", pl, pl * 4, 1, 1, 0, ho, wo, 0)]
-            if b == 0 and (s != 1 or inpl != pl * 4):
-                out.append((bi, 3, pre + "downsample.0.weight", pre + "downsample.1.", inpl, pl * 4, 1, s, 0, h, w, 0))
-            inpl, h, w, bi = pl * 4, ho, wo, bi + 1
+            if basic:
+                out += [(bi, 0, pre + "conv1.weight", pre + "bn1.", inpl, pl, 3, s, 1, h, w, 0),
+                        (bi, 1, pre + "conv2.weight", pre + "bn2.", pl, pl, 3, 1, 1, ho, wo, 0)]
+            else:
+                out += [(bi, 0, pre + "conv1.weight", pre + "bn1.", inpl, pl, 1, 1, 0, h, w, 0),
+                        (bi, 1, pre + "conv2.weight", pre + "bn2.", pl, pl, 3, s, 1, h, w, 0),
+                        (bi, 2, pre + "conv3.weight", pre + "bn3.", pl, pl * 4, 1, 1, 0, ho, wo, 0)]
+            if b == 0 and (s != 1 or inpl != outc):
+                out.append((bi, 3, pre + "downsample.0.weight", pre + "downsample.1.", inpl, outc, 1, s, 0, h, w, 0))
+            inpl, h, w, bi = outc, ho, wo, bi + 1
     return out
 
 
-def make_model(layers):
-    from resnet import ResNet, Bottleneck
+def make_model(layers, basic=False):
+    from resnet import ResNet, BasicBlock, Bottleneck
     torch.manual_seed(0)
-    return ResNet(Bottleneck, list(layers)).to(DEV).train()
+    return ResNet(BasicBlock if basic else Bottleneck, list(layers)).to(DEV).train()
 
 
 def peek_conv(L, net, block, conv):

@@ -1,6 +1,6 @@
 """CPU-only: the test aids of the ResNet runner's batched kernels (include/dirb200.h, "Test aids: the runner's batched
-kernels") and dirb200_resnet_peek_conv refuse bad arguments on the host, with rc -1 and a message, before any CUDA
-call.  Every pointer below is a dummy that must never be dereferenced, so a call that got past its checks would fault
+kernels"), dirb200_resnet_peek_conv and the runner's peeks and backward tap refuse bad arguments on the host, with rc -1
+and a message, before any CUDA call.  Every pointer below is a dummy that must never be dereferenced, so a call that got past its checks would fault
 on a GPU machine and fail without one."""
 import ctypes
 
@@ -173,3 +173,34 @@ def test_peek_refuses_bad_selectors_before_reading_the_net():
     for block, which in ((-1, 0), (-1, 7), (0, 6), (0, 7)):
         refused("dirb200_resnet_peek", None, block, which, *out, msg="null")
         refused("dirb200_resnet_peek", D, block, which, None, ctypes.byref(rows), ctypes.byref(ch), msg="null")
+
+
+def test_peek_bn_coef_refuses_a_null_net_or_output():
+    import resnet  # noqa: F401  (registers the runner bindings)
+    p = ctypes.c_void_p()
+    for block, conv in ((-1, 0), (0, 0), (0, 3)):
+        refused("dirb200_resnet_peek_bn_coef", None, block, conv, ctypes.byref(p), msg="null")
+        refused("dirb200_resnet_peek_bn_coef", D, block, conv, None, msg="null")
+
+
+def test_backward_tap_refuses_a_bad_block_or_a_null_net():
+    """A block below DIRB200_RESNET_NO_TAP (-2) is refused before the net is read; -2 .. blocks-1 need a net."""
+    import resnet  # noqa: F401  (registers the runner bindings)
+    for block in (-3, -100):
+        refused("dirb200_resnet_set_backward_tap", None, block, msg=f"bad block {block}")
+    for block in (-2, -1, 0, 15):
+        refused("dirb200_resnet_set_backward_tap", None, block, msg="null net")
+
+
+def test_peek_backward_refuses_bad_selectors_before_reading_the_net():
+    """dirb200_resnet_peek_backward checks its selector (0 .. 13) before the net, then its pointers."""
+    import resnet  # noqa: F401  (registers the runner bindings)
+    ptr, rows, ch = ctypes.c_void_p(), ctypes.c_int64(), ctypes.c_int()
+    out = (ctypes.byref(ptr), ctypes.byref(rows), ctypes.byref(ch))
+    for which in (-1, 14, 100):
+        refused("dirb200_resnet_peek_backward", None, which, *out, msg=f"bad selector {which}")
+    for which in (0, 3, 13):
+        refused("dirb200_resnet_peek_backward", None, which, *out, msg="null")
+        refused("dirb200_resnet_peek_backward", D, which, None, ctypes.byref(rows), ctypes.byref(ch), msg="null")
+        refused("dirb200_resnet_peek_backward", D, which, ctypes.byref(ptr), None, ctypes.byref(ch), msg="null")
+        refused("dirb200_resnet_peek_backward", D, which, ctypes.byref(ptr), ctypes.byref(rows), None, msg="null")

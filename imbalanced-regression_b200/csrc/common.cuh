@@ -57,6 +57,13 @@ inline int num_sms() {
   return n;
 }
 
+// An A/B switch such as DIRB200_GRAPH: on unless its value starts with '0'.  Each caller keeps the result in a
+// function-local static of its own, so every switch is read once per process.
+inline bool env_switch(const char* name) {
+  const char* e = getenv(name);
+  return !(e != nullptr && e[0] == '0');
+}
+
 __device__ __forceinline__ float warp_sum(float v) {
 #pragma unroll
   for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);

@@ -825,18 +825,12 @@ static int check_shape(const ConvShape& s, bool stem, const char* who) {
 // DIRB200_ATMA=0 keeps the cp.async gather for every layer (A/B measurements); default: 1x1 stride-1 GEMMs take the
 // A operand through TMA.
 static bool atma_enabled() {
-  static const bool on = [] {
-    const char* e = getenv("DIRB200_ATMA");
-    return !(e != nullptr && e[0] == '0');
-  }();
+  static const bool on = env_switch("DIRB200_ATMA");
   return on;
 }
 // DIRB200_IM2COL=0: the cp.async gather for the convs that would take im2col-mode TMA.
 static bool im2col_enabled() {
-  static const bool on = [] {
-    const char* e = getenv("DIRB200_IM2COL");
-    return !(e != nullptr && e[0] == '0');
-  }();
+  static const bool on = env_switch("DIRB200_IM2COL");
   return on && atma_enabled();
 }
 

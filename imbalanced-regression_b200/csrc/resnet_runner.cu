@@ -22,7 +22,8 @@ struct BNLayer {
 };
 
 struct ConvLayer {
-  ConvShape s{};
+  ConvShape s{};    // the GEMM's shape (the stem: the 4x4x16 space-to-depth form)
+  ConvShape ref{};  // the conv as the reference defines it, in the weight layout [cout][cin][kh][kw] (the stem: 3x7x7)
   bool stem = false;
   size_t w_off = 0;
   __nv_bfloat16 *wf = nullptr, *wd = nullptr;  // GEMM operands (fprop / dgrad layouts)
@@ -38,6 +39,7 @@ struct Block {
   ConvLayer c1, c2, c3, ds;    // a basic block has no c3
   bool basic = false;
   bool has_ds = false;
+  int first_conv = 0;          // index of c1 in dirb200_net::convs; c2 [, c3] [, ds] follow
   const __nv_bfloat16* in = nullptr;
   __nv_bfloat16* out = nullptr;
   uint8_t* mask = nullptr;     // ReLU mask of `out`, 1 bit per element ([rows][c/8] bytes), for the backward pass
@@ -46,6 +48,23 @@ struct Block {
   ConvLayer& tail() { return basic ? c2 : c3; }
   const ConvLayer& tail() const { return basic ? c2 : c3; }
   ConvLayer& pre_tail() { return basic ? c1 : c2; }
+};
+
+// Roles of the scratch buffers (each holds any activation of the net).  The first four hold the backward's gradient
+// pairs, whose roles rotate from block to block (BwdBuffers); their names are the roles they start in.  T1 .. T3 hold a
+// block's transient gradients, G3 a layer group's gradient from outside the network, staged at a fixed address.
+enum ScratchRole { kScrGA = 0, kScrSpareB, kScrNA, kScrNB, kScrT1, kScrT2, kScrT3, kScrG3, kNumScratch };
+
+// Where the backward's gradients are between blocks and between stages: the incoming pair (gA, gB) of the next block
+// to run, the pair (nA, nB) that block's input gradients go to, and the buffer that becomes the next nB when the
+// block had no gB (the first block after the gradient enters).
+struct BwdBuffers {
+  __nv_bfloat16 *gA = nullptr, *gB = nullptr, *nA = nullptr, *nB = nullptr, *spareB = nullptr;
+  int gB_h = 0, gB_w = 0;   // > 0: gB is the compact [n, h/2, w/2, c] gradient of a stride-2 1x1 downsample
+  // the state in which the gradient from outside the network enters, into gA
+  static BwdBuffers start(__nv_bfloat16* const* scratch) {
+    return BwdBuffers{scratch[kScrGA], nullptr, scratch[kScrNA], scratch[kScrNB], scratch[kScrSpareB], 0, 0};
+  }
 };
 
 }  // namespace dirb200
@@ -65,42 +84,52 @@ struct dirb200_net {
   uint8_t* pool_idx = nullptr;
   int pool_h = 0, pool_w = 0;
   int feat_c = 0, feat_hw = 0;
-  __nv_bfloat16* scratch[8] = {};
-  WgradReduceDesc* reduce_descs = nullptr;     // device table, conv layers in backward-stage order
-  std::vector<int> reduce_begin;               // first table entry of stage s (0 = stem, 1.. = layer groups); +1 sentinel
+  __nv_bfloat16* scratch[kNumScratch] = {};
+  // every conv in named_parameters() order (stem, then each block's c1, c2 [, c3] [, ds]): the order of the three
+  // device tables below
+  std::vector<ConvLayer*> convs;
+  std::vector<int> conv_begin;   // first conv of backward stage s (0 = stem, 1.. = layer groups); +1 sentinel
+  WgradReduceDesc* reduce_descs = nullptr;  // device table: every conv's split-K reduction, one launch per stage
   float* bn_partial = nullptr;   // per-CTA partial sums of the BN column reductions (backward)
   float* stat_partial = nullptr; // per-CTA BN statistics [CTA][2][c] written by the conv fprop epilogue (conv.cuh)
   PrepDesc* prep_descs = nullptr; // device table for the single weight re-layout launch
-  BnEvalDesc* bn_eval_descs = nullptr;  // device table: every BN layer, for the single eval-coefficient launch
-  int num_bns = 0, max_bn_c = 0;
-  int num_convs = 0;
+  BnEvalDesc* bn_eval_descs = nullptr;  // device table: every conv's BN layer, for the single eval-coefficient launch
+  int max_bn_c = 0;
   size_t param_count = 0, running_count = 0, activation_bytes = 0;
   std::vector<void*> allocs;
   bool forward_was_training = false;
   // backward runs stage by stage (layer4 .. layer1, stem) so that the caller can start the gradient all-reduce of a
   // finished stage while the earlier stages still compute; the incoming-gradient buffers live here between the calls
   std::vector<int> stage_begin;          // first block of stage s (1-based stages; stage_begin[num_stages+1] = #blocks)
-  int bwd_next_stage = -1;               // stage the next dirb200_resnet_backward_stage call must name (-1: none pending)
-  __nv_bfloat16 *bw_gA = nullptr, *bw_gB = nullptr, *bw_nA = nullptr, *bw_nB = nullptr, *bw_spareB = nullptr;
-  int bw_gB_h = 0, bw_gB_w = 0;          // > 0: bw_gB is the compact [n, h/2, w/2, c] gradient of a stride-2 1x1 downsample
+  BwdBuffers bw;
+  struct BwdOrder {
+    int next = -1;         // stage the next backward-stage call must name (-1: none pending)
+    bool blocks = false;   // the pending backward is the multi-scale one
+    int top = -1;          // topmost stage that received a gradient so far (-1: none)
+  } bwd;
   // CUDA graphs of the launch sequences whose pointers never change (the training forward after the input re-layout,
-  // every backward stage after the average-pool backward): captured on the second call, replayed from then on
+  // every backward stage after the gradient enters): captured on the second call, replayed from then on
   struct GraphSlot {
     cudaGraphExec_t exec = nullptr;
     const void *k0 = nullptr, *k1 = nullptr;   // the (params, running / grads) pointers the capture holds
     int warm = 0;
     int64_t launches = 0;                      // kernel launches inside (added to the launch counter per replay)
-    // host-side state the captured calls leave behind (backward stages)
-    __nv_bfloat16 *gA = nullptr, *gB = nullptr, *nA = nullptr, *nB = nullptr, *spareB = nullptr;
-    int gB_h = 0, gB_w = 0;
+    BwdBuffers bw;                             // backward stages: where the captured sequence leaves the gradients
+    void drop() {
+      if (exec) cudaGraphExecDestroy(exec);
+      *this = GraphSlot{};
+    }
   };
-  GraphSlot g_fwd, g_bwd[6];
-  // multi-scale (encoder) mode, dirb200_resnet_forward_blocks / dirb200_resnet_backward_blocks_stage: graphs of their
-  // own.  A backward stage's sequence depends on the topmost stage that received a gradient (it fixes which scratch
-  // buffers hold the incoming pair) and on whether the stage's own block gradient is added: [stage][top][d_block]
-  GraphSlot g_fwd_blocks, g_bwd_blocks[6][6][2];
-  bool bwd_blocks = false;   // the pending backward is the multi-scale one
-  int bwd_top = -1;          // multi-scale backward: topmost stage that received a gradient so far (-1: none)
+  // One slot per launch sequence: the forward and the multi-scale forward, then per backward stage (0 .. 4) the
+  // regression backward's and the multi-scale backward's.  A multi-scale stage's sequence depends on the topmost stage
+  // that received a gradient (it fixes which scratch buffers hold the incoming pair) and on whether the stage's own
+  // block gradient is added.
+  static constexpr int kStages = 5, kSlotsPerStage = 1 + kStages * 2;
+  GraphSlot graphs[2 + kStages * kSlotsPerStage];
+  GraphSlot& fwd_graph(bool blocks) { return graphs[blocks ? 1 : 0]; }
+  GraphSlot& bwd_graph(int stage, bool blocks, int top, bool g3) {
+    return graphs[2 + stage * kSlotsPerStage + (blocks ? 1 + 2 * top + (g3 ? 1 : 0) : 0)];
+  }
   cudaStream_t cap_stream = nullptr;               // capture happens on a private stream (the caller's may be the legacy default stream, which cannot capture)
   float *enc_buf = nullptr, *denc_buf = nullptr;   // fixed-address copies of the forward's output / the backward's input
   // optional per-kernel-class timing (CUDA events around every launch group)
@@ -150,10 +179,11 @@ static bool setup_bn(dirb200_net* net, BNLayer& bn, int c) {
 
 static bool setup_conv(dirb200_net* net, ConvLayer& cv, int n, int h, int w, int cin, int cout, int k, int stride,
                        int pad, bool stem, bool with_act) {
+  net->convs.push_back(&cv);
   cv.stem = stem;
   const int ho = (h + 2 * pad - k) / stride + 1, wo = (w + 2 * pad - k) / stride + 1;
-  if (stem) cv.s = ConvShape{n, h / 2, w / 2, 16, cout, 4, 4, 1, 2, h / 2, w / 2};
-  else cv.s = ConvShape{n, h, w, cin, cout, k, k, stride, pad, ho, wo};
+  cv.ref = ConvShape{n, h, w, cin, cout, k, k, stride, pad, ho, wo};
+  cv.s = stem ? ConvShape{n, h / 2, w / 2, 16, cout, 4, 4, 1, 2, h / 2, w / 2} : cv.ref;
   cv.w_off = net->param_count;
   net->param_count += (size_t)cout * cin * k * k;
   cv.rows = (int64_t)n * ho * wo;
@@ -169,8 +199,19 @@ static bool setup_conv(dirb200_net* net, ConvLayer& cv, int n, int h, int w, int
   return setup_bn(net, cv.bn, cout);
 }
 
+template <typename T>
+static bool upload_table(dirb200_net* net, T*& dev, const std::vector<T>& host) {
+  NET_ALLOC(dev, sizeof(T) * host.size());
+  return cudaMemcpy(dev, host.data(), sizeof(T) * host.size(), cudaMemcpyHostToDevice) == cudaSuccess;
+}
+
 static bool build(dirb200_net* net, const int* blocks_per_stage, int num_stages) {
   const int n = net->n;
+  // net->convs points into the blocks: they must not move
+  int num_blocks = 0;
+  for (int st = 0; st < num_stages; ++st) num_blocks += std::max(blocks_per_stage[st], 0);
+  net->blocks.reserve(num_blocks);
+  net->conv_begin.assign(1, 0);
   // the stem's activation is never materialised: BN + ReLU are fused into the max pool (bn_relu_maxpool_fwd)
   if (!setup_conv(net, net->stem, n, net->h, net->w, 3, 64, 7, 2, 3, true, false)) return false;
   int h = net->h / 2, w = net->w / 2;
@@ -190,10 +231,12 @@ static bool build(dirb200_net* net, const int* blocks_per_stage, int num_stages)
     const int planes = 64 << st;
     const int outc = basic ? planes : planes * 4;    // planes * block.expansion
     net->stage_begin.push_back((int)net->blocks.size());
+    net->conv_begin.push_back((int)net->convs.size());
     for (int b = 0; b < blocks_per_stage[st]; ++b) {
       const int stride = (b == 0 && st > 0) ? 2 : 1;
       net->blocks.emplace_back();
       Block& B = net->blocks.back();
+      B.first_conv = (int)net->convs.size();
       B.in = cur;
       B.basic = basic;
       B.has_ds = (b == 0) && (stride != 1 || inplanes != outc);
@@ -221,67 +264,30 @@ static bool build(dirb200_net* net, const int* blocks_per_stage, int num_stages)
     }
   }
   net->stage_begin.push_back((int)net->blocks.size());
+  net->conv_begin.push_back((int)net->convs.size());
   net->feat_c = inplanes;
   net->feat_hw = h * w;
   net->max_act = max_act;
-  for (int i = 0; i < 8; ++i) NET_ALLOC(net->scratch[i], max_act * 2);
-  {
-    // split-K reduction jobs: every conv owns its partial buffer; one launch reduces a whole backward stage
-    std::vector<WgradReduceDesc> rd;
-    auto addr = [&](const ConvLayer& cv) {
-      rd.push_back(WgradReduceDesc{cv.wpart, cv.w_off, cv.splits, cv.s.cout, cv.stem ? 3 : cv.s.cin,
-                                   cv.stem ? 7 : cv.s.kh, cv.stem ? 7 : cv.s.kw, cv.stem ? 1 : 0});
-    };
-    net->reduce_begin.clear();
-    net->reduce_begin.push_back(0);
-    addr(net->stem);
-    for (int stg = 1; stg <= num_stages; ++stg) {
-      net->reduce_begin.push_back((int)rd.size());
-      for (int bi = net->stage_begin[stg]; bi < net->stage_begin[stg + 1]; ++bi) {
-        Block& B = net->blocks[bi];
-        addr(B.c1); addr(B.c2);
-        if (!B.basic) addr(B.c3);
-        if (B.has_ds) addr(B.ds);
-      }
-    }
-    net->reduce_begin.push_back((int)rd.size());
-    NET_ALLOC(net->reduce_descs, sizeof(WgradReduceDesc) * rd.size());
-    if (cudaMemcpy(net->reduce_descs, rd.data(), sizeof(WgradReduceDesc) * rd.size(), cudaMemcpyHostToDevice) != cudaSuccess)
-      return false;
-  }
+  for (auto& p : net->scratch) NET_ALLOC(p, max_act * 2);
   NET_ALLOC(net->enc_buf, sizeof(float) * (size_t)n * net->feat_c);
   NET_ALLOC(net->denc_buf, sizeof(float) * (size_t)n * net->feat_c);
   NET_ALLOC(net->bn_partial, sizeof(float) * bn_partial_floats(net->feat_c));
   NET_ALLOC(net->stat_partial, sizeof(float) * bn_partial_floats(net->feat_c));
-  std::vector<PrepDesc> descs;
-  auto add = [&](const ConvLayer& cv) {
-    descs.push_back(make_prep_desc(cv.w_off, cv.s.cout, cv.stem ? 3 : cv.s.cin, cv.stem ? 7 : cv.s.kh, cv.stem ? 7 : cv.s.kw,
-                                   cv.stem ? 1 : 0, cv.wf, cv.wd));
-  };
-  add(net->stem);
-  for (Block& B : net->blocks) {
-    add(B.c1); add(B.c2);
-    if (!B.basic) add(B.c3);
-    if (B.has_ds) add(B.ds);
-  }
-  net->num_convs = (int)descs.size();
-  NET_ALLOC(net->prep_descs, sizeof(PrepDesc) * descs.size());
-  if (cudaMemcpy(net->prep_descs, descs.data(), sizeof(PrepDesc) * descs.size(), cudaMemcpyHostToDevice) != cudaSuccess)
-    return false;
-  std::vector<BnEvalDesc> bd;
-  auto addbn = [&](const BNLayer& bn) {
-    bd.push_back(BnEvalDesc{bn.c, bn.gamma_off, bn.beta_off, bn.rm_off, bn.rv_off, bn.scale, bn.shift});
+  // the weight prep, the split-K reduction (every conv owns its partial buffer; one launch reduces a whole backward
+  // stage) and the eval BN coefficients each run over every conv in one launch
+  std::vector<PrepDesc> prep;
+  std::vector<WgradReduceDesc> reduce;
+  std::vector<BnEvalDesc> bn_eval;
+  for (const ConvLayer* cv : net->convs) {
+    const ConvShape& r = cv->ref;
+    const BNLayer& bn = cv->bn;
+    prep.push_back(make_prep_desc(cv->w_off, r.cout, r.cin, r.kh, r.kw, cv->stem ? 1 : 0, cv->wf, cv->wd));
+    reduce.push_back(WgradReduceDesc{cv->wpart, cv->w_off, cv->splits, r.cout, r.cin, r.kh, r.kw, cv->stem ? 1 : 0});
+    bn_eval.push_back(BnEvalDesc{bn.c, bn.gamma_off, bn.beta_off, bn.rm_off, bn.rv_off, bn.scale, bn.shift});
     net->max_bn_c = std::max(net->max_bn_c, bn.c);
-  };
-  addbn(net->stem.bn);
-  for (Block& B : net->blocks) {
-    addbn(B.c1.bn); addbn(B.c2.bn);
-    if (!B.basic) addbn(B.c3.bn);
-    if (B.has_ds) addbn(B.ds.bn);
   }
-  net->num_bns = (int)bd.size();
-  NET_ALLOC(net->bn_eval_descs, sizeof(BnEvalDesc) * bd.size());
-  return cudaMemcpy(net->bn_eval_descs, bd.data(), sizeof(BnEvalDesc) * bd.size(), cudaMemcpyHostToDevice) == cudaSuccess;
+  return upload_table(net, net->prep_descs, prep) && upload_table(net, net->reduce_descs, reduce) &&
+         upload_table(net, net->bn_eval_descs, bn_eval);
 }
 
 #define RUN(expr)                    \
@@ -324,10 +330,7 @@ static inline void prof_end(dirb200_net* net, cudaStream_t st) {
 // DIRB200_FUSED_STATS=0: batch statistics by the separate bn_stats pass over y (A/B measurements) instead of the
 // conv epilogue.
 static bool fused_stats() {
-  static const bool on = [] {
-    const char* e = getenv("DIRB200_FUSED_STATS");
-    return !(e != nullptr && e[0] == '0');
-  }();
+  static const bool on = env_switch("DIRB200_FUSED_STATS");
   return on;
 }
 
@@ -366,7 +369,7 @@ static int wgrad_step(dirb200_net* net, const __nv_bfloat16* x, const __nv_bfloa
 }
 
 static int wgrad_reduce_stage(dirb200_net* net, int stage, float* grads, cudaStream_t st) {
-  const int lo = net->reduce_begin[stage], hi = net->reduce_begin[stage + 1];
+  const int lo = net->conv_begin[stage], hi = net->conv_begin[stage + 1];
   RUNP(kWgradReduce, wgrad_reduce_all(net->reduce_descs + lo, hi - lo, grads, st));
   return DIRB200_OK;
 }
@@ -398,17 +401,14 @@ static int conv_bn_backward(dirb200_net* net, ConvLayer& cv, const __nv_bfloat16
 // conv -> BN [-> ReLU] and the whole tail conv -> BN -> (+ shortcut) -> ReLU of a block is ONE launch, and no raw conv
 // output is written.  ~58 launches instead of ~165.  DIRB200_FOLDED_EVAL=0 keeps the unfused sequence (A/B checks).
 static bool folded_eval() {
-  static const bool on = [] {
-    const char* e = getenv("DIRB200_FOLDED_EVAL");
-    return !(e != nullptr && e[0] == '0');
-  }();
+  static const bool on = env_switch("DIRB200_FOLDED_EVAL");
   return on;
 }
 
 // enc_out == nullptr: no average pool (multi-scale mode reads the block outputs)
 static int forward_eval_folded(dirb200_net* net, const float* params, const float* running, float* enc_out,
                                cudaStream_t st) {
-  RUNP(kBnStats, bn_eval_coeffs_all(net->bn_eval_descs, net->num_bns, net->max_bn_c, params, running, 1e-5f, st));
+  RUNP(kBnStats, bn_eval_coeffs_all(net->bn_eval_descs, (int)net->convs.size(), net->max_bn_c, params, running, 1e-5f, st));
   // stem: plain conv, then BN + ReLU inside the max pool (as in training; the activation is never materialised)
   RUNP(kFprop, conv_fprop(net->x_s2d, net->stem.wf, net->stem.y, net->stem.s, true, st));
   RUNP(kPool, bn_relu_maxpool_fwd(net->stem.y, net->stem.bn.scale, net->stem.bn.shift, net->n, net->stem.s.ho,
@@ -469,10 +469,7 @@ static int check_blocks_mode(const dirb200_net* net, const char* who) {
 // GraphSlot), which removes the dependent-launch gaps of a stream (A/B on an H100 80GB HBM3 at a 400 W power limit,
 // bench.py batch 256, two runs each: 41.6 ms per step with graphs, 42.1 ms eager).  DIRB200_GRAPH=0 launches eagerly.
 static bool graphs_enabled() {
-  static const bool on = [] {
-    const char* e = getenv("DIRB200_GRAPH");
-    return !(e != nullptr && e[0] == '0');
-  }();
+  static const bool on = env_switch("DIRB200_GRAPH");
   return on;
 }
 
@@ -487,11 +484,7 @@ static int run_graphed(dirb200_net* net, dirb200_net::GraphSlot& g, const void* 
     g_launches.fetch_add(g.launches);
     return DIRB200_OK;
   }
-  if (g.exec) {
-    cudaGraphExecDestroy(g.exec);
-    g.exec = nullptr;
-    g.warm = 0;
-  }
+  if (g.exec) g.drop();
   if (g.warm == 0 || g.k0 != k0 || g.k1 != k1) {
     g.k0 = k0; g.k1 = k1; g.warm = 1;
     return body(st);
@@ -524,10 +517,7 @@ static int run_graphed(dirb200_net* net, dirb200_net::GraphSlot& g, const void* 
 
 // DIRB200_FUSED_BWD_MOMENTS=0: separate bn_bwd_reduce passes everywhere (A/B measurements).
 static bool fused_bwd_moments() {
-  static const bool on = [] {
-    const char* e = getenv("DIRB200_FUSED_BWD_MOMENTS");
-    return !(e != nullptr && e[0] == '0');
-  }();
+  static const bool on = env_switch("DIRB200_FUSED_BWD_MOMENTS");
   return on;
 }
 
@@ -543,6 +533,33 @@ static int dgrad_with_bn_moments(dirb200_net* net, const __nv_bfloat16* dy, Conv
   }
   const DgradBnMoments bm{prev.y, prev.bn.scale, prev.bn.shift, net->bn_partial, lay};
   RUNP(kDgrad, conv_dgrad(dy, cv.wd, g, cv.s, st, &bm));
+  return DIRB200_OK;
+}
+
+// The forward of both modes: the regression's writes enc_out (average pool), the multi-scale one block_out[] (the
+// group outputs).  Each mode's training sequence has a graph slot of its own.
+static int forward(dirb200_net* net, const float* x_nchw, const float* params, float* bn_running, bool tr,
+                   float* enc_out, void* const* block_out, cudaStream_t st) {
+  RUNP(kPrep, prep_weights_all(params, net->prep_descs, (int)net->convs.size(), st));
+  RUNP(kPrep, input_to_s2d(x_nchw, net->n, net->h, net->w, net->x_s2d, st));
+  if (!tr && folded_eval()) {
+    RUN(forward_eval_folded(net, params, bn_running, enc_out, st));
+  } else {
+    // a graph writes the fixed enc_buf
+    float* enc = enc_out && tr && graphs_enabled() && !net->profiling ? net->enc_buf : enc_out;
+    auto body = [&](cudaStream_t st) -> int { return forward_body(net, params, bn_running, tr, enc, st); };
+    if (tr) RUN(run_graphed(net, net->fwd_graph(block_out != nullptr), params, bn_running, st, body));
+    else RUN(body(st));
+    if (enc != enc_out)
+      DIRB_CUDA(cudaMemcpyAsync(enc_out, enc, sizeof(float) * (size_t)net->n * net->feat_c, cudaMemcpyDeviceToDevice,
+                                st));
+  }
+  for (int s = 0; block_out && s < (int)net->stage_begin.size() - 2; ++s) {
+    const Block& B = net->blocks[net->stage_begin[s + 2] - 1];
+    DIRB_CUDA(cudaMemcpyAsync(block_out[s], B.out, sizeof(__nv_bfloat16) * (size_t)B.tail().rows * B.tail().s.cout,
+                              cudaMemcpyDeviceToDevice, st));
+  }
+  net->forward_was_training = tr;
   return DIRB200_OK;
 }
 
@@ -589,14 +606,7 @@ int dirb200_resnet_create_ex(int n, int h, int w, int block, const int* blocks_p
 void dirb200_resnet_destroy(dirb200_net* net) {
   if (!net) return;
   if (net->cap_stream) cudaStreamDestroy(net->cap_stream);
-  if (net->g_fwd.exec) cudaGraphExecDestroy(net->g_fwd.exec);
-  if (net->g_fwd_blocks.exec) cudaGraphExecDestroy(net->g_fwd_blocks.exec);
-  for (auto& g : net->g_bwd)
-    if (g.exec) cudaGraphExecDestroy(g.exec);
-  for (auto& per_stage : net->g_bwd_blocks)
-    for (auto& per_top : per_stage)
-      for (auto& g : per_top)
-        if (g.exec) cudaGraphExecDestroy(g.exec);
+  for (auto& g : net->graphs) g.drop();
   for (void* p : net->allocs) cudaFree(p);
   delete net;
 }
@@ -638,27 +648,7 @@ int dirb200_resnet_forward(dirb200_net* net, const float* x_nchw, const float* p
                            float* enc_out, void* stream) {
   DIRB_CHECK_ARG(net && x_nchw && params && enc_out, "resnet_forward: null pointer");
   DIRB_CHECK_ARG(training || bn_running, "resnet_forward: eval mode needs the running statistics");
-  cudaStream_t st = as_stream(stream);
-  const bool tr = training != 0;
-  RUNP(kPrep, prep_weights_all(params, net->prep_descs, net->num_convs, st));
-  RUNP(kPrep, input_to_s2d(x_nchw, net->n, net->h, net->w, net->x_s2d, st));
-  if (!tr && folded_eval()) {
-    RUN(forward_eval_folded(net, params, bn_running, enc_out, st));
-    net->forward_was_training = false;
-    return DIRB200_OK;
-  }
-  const bool graphed = tr && graphs_enabled() && !net->profiling;
-  float* enc_dst = graphed ? net->enc_buf : enc_out;
-  auto body = [&](cudaStream_t st) -> int { return forward_body(net, params, bn_running, tr, enc_dst, st); };
-  if (graphed) {
-    RUN(run_graphed(net, net->g_fwd, params, bn_running, st, body));
-    DIRB_CUDA(cudaMemcpyAsync(enc_out, net->enc_buf, sizeof(float) * (size_t)net->n * net->feat_c,
-                              cudaMemcpyDeviceToDevice, st));
-  } else {
-    RUN(body(st));
-  }
-  net->forward_was_training = tr;
-  return DIRB200_OK;
+  return forward(net, x_nchw, params, bn_running, training != 0, enc_out, nullptr, as_stream(stream));
 }
 
 /* The same forward without the average pool (nyud2-dir/models/modules.py:33-58, E_resnet.forward): the output of the
@@ -672,24 +662,7 @@ int dirb200_resnet_forward_blocks(dirb200_net* net, const float* x_nchw, const f
   const int nst = (int)net->stage_begin.size() - 2;
   for (int s = 0; s < nst; ++s) DIRB_CHECK_ARG(block_out[s], "resnet_forward_blocks: null block_out[%d]", s);
   RUN(check_blocks_mode(net, "resnet_forward_blocks"));
-  cudaStream_t st = as_stream(stream);
-  const bool tr = training != 0;
-  RUNP(kPrep, prep_weights_all(params, net->prep_descs, net->num_convs, st));
-  RUNP(kPrep, input_to_s2d(x_nchw, net->n, net->h, net->w, net->x_s2d, st));
-  if (!tr && folded_eval()) {
-    RUN(forward_eval_folded(net, params, bn_running, nullptr, st));
-  } else {
-    auto body = [&](cudaStream_t st) -> int { return forward_body(net, params, bn_running, tr, nullptr, st); };
-    if (tr) RUN(run_graphed(net, net->g_fwd_blocks, params, bn_running, st, body));
-    else RUN(body(st));
-  }
-  for (int s = 0; s < nst; ++s) {
-    const Block& B = net->blocks[net->stage_begin[s + 2] - 1];
-    DIRB_CUDA(cudaMemcpyAsync(block_out[s], B.out, sizeof(__nv_bfloat16) * (size_t)B.tail().rows * B.tail().s.cout,
-                              cudaMemcpyDeviceToDevice, st));
-  }
-  net->forward_was_training = tr;
-  return DIRB200_OK;
+  return forward(net, x_nchw, params, bn_running, training != 0, nullptr, block_out, as_stream(stream));
 }
 
 }  // extern "C"
@@ -710,13 +683,12 @@ static int tap_copy(dirb200_net* net, int block, int which, const __nv_bfloat16*
   return DIRB200_OK;
 }
 
-// blocks [lo, hi) in reverse order; the incoming gradient pair is net->bw_gA / bw_gB, plus g3 (may be null) for the
+// blocks [lo, hi) in reverse order; the incoming gradient pair is net->bw.gA / gB, plus g3 (may be null) for the
 // output of block hi-1 (multi-scale mode: the gradient of a layer group's output from outside the network)
 static int backward_blocks(dirb200_net* net, int lo, int hi, const float* params, float* grads, cudaStream_t st,
-                           const __nv_bfloat16* g3 = nullptr) {
-  __nv_bfloat16 *gA = net->bw_gA, *gB = net->bw_gB, *nA = net->bw_nA, *nB = net->bw_nB, *spareB = net->bw_spareB;
-  __nv_bfloat16 *t1 = net->scratch[4], *t2 = net->scratch[5], *t3 = net->scratch[6];
-  int gB_h = net->bw_gB_h, gB_w = net->bw_gB_w;
+                           const __nv_bfloat16* g3) {
+  BwdBuffers bw = net->bw;
+  __nv_bfloat16 *t1 = net->scratch[kScrT1], *t2 = net->scratch[kScrT2], *t3 = net->scratch[kScrT3];
   for (int bi = hi - 1; bi >= lo; --bi) {
     Block& B = net->blocks[bi];
     ConvLayer& T = B.tail();       // conv3 (bottleneck) / conv2 (basic block)
@@ -726,15 +698,15 @@ static int backward_blocks(dirb200_net* net, int lo, int hi, const float* params
     int nblk = 0;
     const int kparts = B.has_ds ? 3 : 2;
     const int n = T.s.n;
-    RUN(tap_copy(net, bi, kTapGA, gA, T.rows, b3.c, st));
-    RUN(tap_copy(net, bi, kTapGB, gB, gB_h ? (int64_t)n * (gB_h / 2) * (gB_w / 2) : T.rows, b3.c, st));
+    RUN(tap_copy(net, bi, kTapGA, bw.gA, T.rows, b3.c, st));
+    RUN(tap_copy(net, bi, kTapGB, bw.gB, bw.gB_h ? (int64_t)n * (bw.gB_h / 2) * (bw.gB_w / 2) : T.rows, b3.c, st));
     if (bi == hi - 1) RUN(tap_copy(net, bi, kTapG3, g3, T.rows, b3.c, st));
     // identity blocks: the reduction also stores dz (= the gradient of the shortcut path, nB) so that the apply pass
     // reads ONE gradient tensor instead of gA, gB and the mask again
-    RUNP(kBnBwdReduce, bn_bwd_reduce(gA, gB, T.y, B.has_ds ? B.ds.y : nullptr, nullptr, nullptr, B.mask, T.rows,
-                                     b3.c, net->bn_partial, &nblk, st, gB_h, gB_w, B.has_ds ? nullptr : nB,
+    RUNP(kBnBwdReduce, bn_bwd_reduce(bw.gA, bw.gB, T.y, B.has_ds ? B.ds.y : nullptr, nullptr, nullptr, B.mask, T.rows,
+                                     b3.c, net->bn_partial, &nblk, st, bw.gB_h, bw.gB_w, B.has_ds ? nullptr : bw.nB,
                                      bi == hi - 1 ? g3 : nullptr));
-    if (!B.has_ds) RUN(tap_copy(net, bi, kTapDz, nB, T.rows, b3.c, st));
+    if (!B.has_ds) RUN(tap_copy(net, bi, kTapDz, bw.nB, T.rows, b3.c, st));
     if (B.has_ds) {
       BNLayer& bd = B.ds.bn;
       RUNP(kBnBwdApply, bn_bwd_coeffs(net->bn_partial, nblk, kparts, 2, T.rows, b3.c, bd.mean, bd.invstd,
@@ -743,14 +715,14 @@ static int backward_blocks(dirb200_net* net, int lo, int hi, const float* params
     RUNP(kBnBwdApply, bn_bwd_coeffs(net->bn_partial, nblk, kparts, 1, T.rows, b3.c, b3.mean, b3.invstd,
                                     params + b3.gamma_off, grads + b3.gamma_off, grads + b3.beta_off, b3.coef, st));
     if (B.has_ds)
-      RUNP(kBnBwdApply, bn_bwd_apply(gA, gB, T.y, b3.coef, B.ds.y, B.ds.bn.coef, nullptr, nullptr, B.mask, T.rows,
-                                     b3.c, t1, t2, nullptr, st, gB_h, gB_w));
+      RUNP(kBnBwdApply, bn_bwd_apply(bw.gA, bw.gB, T.y, b3.coef, B.ds.y, B.ds.bn.coef, nullptr, nullptr, B.mask, T.rows,
+                                     b3.c, t1, t2, nullptr, st, bw.gB_h, bw.gB_w));
     else
-      RUNP(kBnBwdApply, bn_bwd_apply(nB, nullptr, T.y, b3.coef, nullptr, nullptr, nullptr, nullptr, nullptr, T.rows,
+      RUNP(kBnBwdApply, bn_bwd_apply(bw.nB, nullptr, T.y, b3.coef, nullptr, nullptr, nullptr, nullptr, nullptr, T.rows,
                                      b3.c, t1, nullptr, nullptr, st));
     RUN(tap_copy(net, bi, kTapDyTail, t1, T.rows, b3.c, st));
     if (B.has_ds) RUN(tap_copy(net, bi, kTapDyDs, t2, T.rows, b3.c, st));
-    gB_h = gB_w = 0;
+    bw.gB_h = bw.gB_w = 0;
     // ---- tail conv
     RUN(wgrad_step(net, M.a, t1, T, st));
     StatLayout mlay{};
@@ -769,8 +741,8 @@ static int backward_blocks(dirb200_net* net, int lo, int hi, const float* params
     }
     // ---- conv1 (bn1 is done: t1 = the gradient of its output)
     RUN(wgrad_step(net, B.in, t1, B.c1, st));
-    RUNP(kDgrad, conv_dgrad(t1, B.c1.wd, nA, B.c1.s, st));
-    RUN(tap_copy(net, bi, kTapNA, nA, (int64_t)n * B.c1.s.h * B.c1.s.w, B.c1.s.cin, st));
+    RUNP(kDgrad, conv_dgrad(t1, B.c1.wd, bw.nA, B.c1.s, st));
+    RUN(tap_copy(net, bi, kTapNA, bw.nA, (int64_t)n * B.c1.s.h * B.c1.s.w, B.c1.s.cin, st));
     // ---- downsample branch
     if (B.has_ds) {
       RUN(wgrad_step(net, B.in, t2, B.ds, st));
@@ -781,24 +753,23 @@ static int backward_blocks(dirb200_net* net, int lo, int hi, const float* params
         // ([n, h/2, w/2, cin], a plain GEMM over the strided grid); the previous block's output BN backward adds it at
         // the even positions (no memset of the full map, no scattered store, no dense re-reads of zeros)
         const ConvShape cs{d.n, d.ho, d.wo, d.cin, d.cout, 1, 1, 1, 0, d.ho, d.wo};
-        RUNP(kDgrad, conv_dgrad(t2, B.ds.wd, nB, cs, st));
-        RUN(tap_copy(net, bi, kTapNB, nB, (int64_t)n * d.ho * d.wo, d.cin, st));
-        gB_h = d.h;
-        gB_w = d.w;
+        RUNP(kDgrad, conv_dgrad(t2, B.ds.wd, bw.nB, cs, st));
+        RUN(tap_copy(net, bi, kTapNB, bw.nB, (int64_t)n * d.ho * d.wo, d.cin, st));
+        bw.gB_h = d.h;
+        bw.gB_w = d.w;
       } else {
-        RUNP(kDgrad, conv_dgrad(t2, B.ds.wd, nB, B.ds.s, st));
-        RUN(tap_copy(net, bi, kTapNB, nB, (int64_t)n * d.h * d.w, d.cin, st));
+        RUNP(kDgrad, conv_dgrad(t2, B.ds.wd, bw.nB, B.ds.s, st));
+        RUN(tap_copy(net, bi, kTapNB, bw.nB, (int64_t)n * d.h * d.w, d.cin, st));
       }
     }
     // the two gradients w.r.t. this block's input become the next (earlier) block's incoming pair
-    __nv_bfloat16* oldA = gA;
-    __nv_bfloat16* oldB = gB ? gB : spareB;
-    gA = nA; gB = nB;
-    nA = oldA; nB = oldB;
-    spareB = nullptr;
+    __nv_bfloat16* oldA = bw.gA;
+    __nv_bfloat16* oldB = bw.gB ? bw.gB : bw.spareB;
+    bw.gA = bw.nA; bw.gB = bw.nB;
+    bw.nA = oldA; bw.nB = oldB;
+    bw.spareB = nullptr;
   }
-  net->bw_gA = gA; net->bw_gB = gB; net->bw_nA = nA; net->bw_nB = nB; net->bw_spareB = spareB;
-  net->bw_gB_h = gB_h; net->bw_gB_w = gB_w;
+  net->bw = bw;
   return DIRB200_OK;
 }
 
@@ -812,11 +783,11 @@ static int backward_stage_run(dirb200_net* net, int stage, const float* params, 
       RUN(backward_blocks(net, net->stage_begin[stage], net->stage_begin[stage + 1], params, grads, st, g3));
     } else {
       // ---- stem: maxpool -> bn1+relu -> conv1 (no data gradient needed)
-      __nv_bfloat16 *t1 = net->scratch[4], *t3 = net->scratch[6];
+      __nv_bfloat16 *t1 = net->scratch[kScrT1], *t3 = net->scratch[kScrT3];
       const int64_t pool_rows = (int64_t)net->n * net->pool_h * net->pool_w;
-      RUN(tap_copy(net, -1, kTapGA, net->bw_gA, pool_rows, 64, st));
-      RUN(tap_copy(net, -1, kTapGB, net->bw_gB, pool_rows, 64, st));
-      RUNP(kPool, maxpool_bwd(net->bw_gA, net->bw_gB, net->pool_idx, net->n, net->stem.s.ho, net->stem.s.wo, 64, t3, st));
+      RUN(tap_copy(net, -1, kTapGA, net->bw.gA, pool_rows, 64, st));
+      RUN(tap_copy(net, -1, kTapGB, net->bw.gB, pool_rows, 64, st));
+      RUNP(kPool, maxpool_bwd(net->bw.gA, net->bw.gB, net->pool_idx, net->n, net->stem.s.ho, net->stem.s.wo, 64, t3, st));
       RUN(tap_copy(net, -1, kTapPool, t3, net->stem.rows, 64, st));
       RUN(conv_bn_backward(net, net->stem, t3, params, grads, t1, st));
       RUN(tap_copy(net, -1, kTapDyStem, t1, net->stem.rows, 64, st));
@@ -829,13 +800,57 @@ static int backward_stage_run(dirb200_net* net, int stage, const float* params, 
   if (!graphs_enabled() || net->profiling || net->tap_block != DIRB200_RESNET_NO_TAP) return body(st);
   const bool replay = g.exec && g.k0 == params && g.k1 == grads;
   RUN(run_graphed(net, g, params, grads, st, body));
-  if (replay) {
-    net->bw_gA = g.gA; net->bw_gB = g.gB; net->bw_nA = g.nA; net->bw_nB = g.nB; net->bw_spareB = g.spareB;
-    net->bw_gB_h = g.gB_h; net->bw_gB_w = g.gB_w;
-  } else {
-    g.gA = net->bw_gA; g.gB = net->bw_gB; g.nA = net->bw_nA; g.nB = net->bw_nB; g.spareB = net->bw_spareB;
-    g.gB_h = net->bw_gB_h; g.gB_w = net->bw_gB_w;
+  if (replay) net->bw = g.bw;
+  else g.bw = net->bw;
+  return DIRB200_OK;
+}
+
+// One backward stage of either mode (dirb200_resnet_backward_stage, dirb200_resnet_backward_blocks_stage): the order
+// checks, the entry of the gradient from outside the network, then the stage's own launches.
+static int backward_stage(dirb200_net* net, bool blocks, int stage, const float* d_enc, const void* d_block,
+                          const float* params, float* grads, cudaStream_t st) {
+  const char* who = blocks ? "resnet_backward_blocks_stage" : "resnet_backward_stage";
+  DIRB_CHECK_ARG(net && params && grads, "%s: null pointer", who);
+  const int nst = (int)net->stage_begin.size() - 2;
+  DIRB_CHECK_ARG(stage >= 0 && stage <= nst, "%s: bad stage %d", who, stage);
+  if (blocks) {
+    DIRB_CHECK_ARG(stage > 0 || !d_block, "%s: stage 0 (the stem) takes no block gradient", who);
+    RUN(check_blocks_mode(net, who));
   }
+  dirb200_net::BwdOrder& o = net->bwd;
+  if (stage == nst) {
+    DIRB_CHECK_ARG(net->forward_was_training, "%s: needs a preceding training-mode forward",
+                   blocks ? who : "resnet_backward");
+    DIRB_CHECK_ARG(blocks || d_enc, "%s: the first stage needs d_enc", who);
+    o.top = -1;
+    net->tap_written = 0;
+  } else {
+    DIRB_CHECK_ARG(o.next == stage && o.blocks == blocks, "%s: stage %d out of order (expected %d%s)", who, stage,
+                   o.next, o.blocks != blocks ? " of a multi-scale backward" : "");
+  }
+  o.next = -1;
+  o.blocks = blocks;
+  // the gradient from outside the network: the regression's d_enc at the top stage, a group output's d_block
+  const __nv_bfloat16* g3 = nullptr;
+  if (blocks ? stage > 0 && d_block : stage == nst) {
+    const ConvLayer& T = net->blocks[net->stage_begin[stage + 1] - 1].tail();
+    const size_t bytes = sizeof(__nv_bfloat16) * (size_t)T.rows * T.s.cout;
+    if (o.top < 0) {
+      // the first gradient of this backward enters into gA
+      o.top = stage;
+      net->bw = BwdBuffers::start(net->scratch);
+      if (blocks) DIRB_CUDA(cudaMemcpyAsync(net->bw.gA, d_block, bytes, cudaMemcpyDeviceToDevice, st));
+      else RUNP(kPool, avgpool_bwd(d_enc, net->n, net->feat_hw, net->feat_c, net->bw.gA, st));
+    } else {
+      // a third operand of the group output's BN-backward reduction, staged at a fixed address for the graph
+      DIRB_CUDA(cudaMemcpyAsync(net->scratch[kScrG3], d_block, bytes, cudaMemcpyDeviceToDevice, st));
+      g3 = net->scratch[kScrG3];
+    }
+  }
+  // a stage that no gradient has reached yet (multi-scale mode) does nothing
+  if (o.top >= 0) RUN(backward_stage_run(net, stage, params, grads, g3, net->bwd_graph(stage, blocks, o.top, g3), st));
+  o.next = stage - 1;          // -1 after the stem: nothing pending
+  if (stage == 0) o.blocks = false;
   return DIRB200_OK;
 }
 
@@ -851,28 +866,7 @@ extern "C" {
  * gradient reduction, here overlapped).  d_enc is only read by the first call. */
 int dirb200_resnet_backward_stage(dirb200_net* net, int stage, const float* d_enc, const float* params, float* grads,
                                   void* stream) {
-  DIRB_CHECK_ARG(net && params && grads, "resnet_backward_stage: null pointer");
-  const int nst = (int)net->stage_begin.size() - 2;
-  DIRB_CHECK_ARG(stage >= 0 && stage <= nst, "resnet_backward_stage: bad stage %d", stage);
-  cudaStream_t st = as_stream(stream);
-  if (stage == nst) {
-    DIRB_CHECK_ARG(net->forward_was_training, "resnet_backward: needs a preceding training-mode forward");
-    DIRB_CHECK_ARG(d_enc, "resnet_backward_stage: the first stage needs d_enc");
-    net->tap_written = 0;
-    net->bw_gA = net->scratch[0]; net->bw_gB = nullptr; net->bw_nA = net->scratch[2]; net->bw_nB = net->scratch[3];
-    net->bw_spareB = net->scratch[1];
-    net->bw_gB_h = net->bw_gB_w = 0;
-    RUNP(kPool, avgpool_bwd(d_enc, net->n, net->feat_hw, net->feat_c, net->bw_gA, st));
-  } else {
-    DIRB_CHECK_ARG(net->bwd_next_stage == stage && !net->bwd_blocks,
-                   "resnet_backward_stage: stage %d out of order (expected %d%s)", stage, net->bwd_next_stage,
-                   net->bwd_blocks ? " of a multi-scale backward" : "");
-  }
-  net->bwd_next_stage = -1;
-  net->bwd_blocks = false;
-  RUN(backward_stage_run(net, stage, params, grads, nullptr, net->g_bwd[stage], st));
-  net->bwd_next_stage = stage - 1;          // -1 after the stem: nothing pending
-  return DIRB200_OK;
+  return backward_stage(net, false, stage, d_enc, nullptr, params, grads, as_stream(stream));
 }
 
 /* Multi-scale backward (nyud2-dir/models/modules.py:33-58, E_resnet.forward): stage = num_stages first, then
@@ -881,45 +875,7 @@ int dirb200_resnet_backward_stage(dirb200_net* net, int stage, const float* d_en
  * nor from the stages above, does nothing: its parameter gradients keep their values. */
 int dirb200_resnet_backward_blocks_stage(dirb200_net* net, int stage, const void* d_block, const float* params,
                                          float* grads, void* stream) {
-  DIRB_CHECK_ARG(net && params && grads, "resnet_backward_blocks_stage: null pointer");
-  const int nst = (int)net->stage_begin.size() - 2;
-  DIRB_CHECK_ARG(stage >= 0 && stage <= nst, "resnet_backward_blocks_stage: bad stage %d", stage);
-  DIRB_CHECK_ARG(stage > 0 || !d_block, "resnet_backward_blocks_stage: stage 0 (the stem) takes no block gradient");
-  RUN(check_blocks_mode(net, "resnet_backward_blocks_stage"));
-  cudaStream_t st = as_stream(stream);
-  if (stage == nst) {
-    DIRB_CHECK_ARG(net->forward_was_training, "resnet_backward_blocks_stage: needs a preceding training-mode forward");
-    net->bwd_top = -1;
-    net->tap_written = 0;
-  } else {
-    DIRB_CHECK_ARG(net->bwd_next_stage == stage && net->bwd_blocks,
-                   "resnet_backward_blocks_stage: stage %d out of order (expected %d%s)", stage, net->bwd_next_stage,
-                   net->bwd_blocks ? "" : " of a multi-scale backward");
-  }
-  net->bwd_next_stage = -1;
-  net->bwd_blocks = true;
-  const __nv_bfloat16* g3 = nullptr;
-  if (stage > 0 && d_block) {
-    const ConvLayer& T = net->blocks[net->stage_begin[stage + 1] - 1].tail();
-    const size_t bytes = sizeof(__nv_bfloat16) * (size_t)T.rows * T.s.cout;
-    if (net->bwd_top < 0) {
-      // the first gradient of this backward: it enters like the average-pool backward's output does
-      net->bwd_top = stage;
-      net->bw_gA = net->scratch[0]; net->bw_gB = nullptr; net->bw_nA = net->scratch[2]; net->bw_nB = net->scratch[3];
-      net->bw_spareB = net->scratch[1];
-      net->bw_gB_h = net->bw_gB_w = 0;
-      DIRB_CUDA(cudaMemcpyAsync(net->bw_gA, d_block, bytes, cudaMemcpyDeviceToDevice, st));
-    } else {
-      // a third operand of the group output's BN-backward reduction, staged at a fixed address for the graph
-      DIRB_CUDA(cudaMemcpyAsync(net->scratch[7], d_block, bytes, cudaMemcpyDeviceToDevice, st));
-      g3 = net->scratch[7];
-    }
-  }
-  if (net->bwd_top >= 0)
-    RUN(backward_stage_run(net, stage, params, grads, g3, net->g_bwd_blocks[stage][net->bwd_top][g3 ? 1 : 0], st));
-  net->bwd_next_stage = stage - 1;
-  if (stage == 0) net->bwd_blocks = false;
-  return DIRB200_OK;
+  return backward_stage(net, true, stage, nullptr, d_block, params, grads, as_stream(stream));
 }
 
 /* Parameters of stage `stage` (0 = stem conv1 + bn1, s = layer group s) occupy [*lo, *hi) of the flat buffers. */
@@ -928,9 +884,9 @@ int dirb200_resnet_stage_param_range(const dirb200_net* net, int stage, int64_t*
   const int nst = (int)net->stage_begin.size() - 2;
   DIRB_CHECK_ARG(stage >= 0 && stage <= nst, "resnet_stage_param_range: bad stage %d", stage);
   auto first = [&](int s) -> int64_t {
-    return s > nst ? (int64_t)net->param_count : (int64_t)net->blocks[net->stage_begin[s]].c1.w_off;
+    return s > nst ? (int64_t)net->param_count : (int64_t)net->convs[net->conv_begin[s]]->w_off;
   };
-  *lo = stage == 0 ? 0 : first(stage);
+  *lo = first(stage);
   *hi = first(stage + 1);
   return DIRB200_OK;
 }
@@ -1000,25 +956,20 @@ int dirb200_resnet_peek(dirb200_net* net, int block, int which, void** ptr, int6
 /* Test / debugging aid: one conv layer's buffers, offset, shape and the split factor of its reduction-table entry.
  * block = -1: stem (conv 0); block >= 0: conv 0 / 1 / 2 / 3 = conv1 / conv2 / conv3 / downsample (conv 2 refused for a
  * basic block). */
-// The conv layer (block, conv) names and its entry in the split-K reduction table; `who` prefixes the refusals.
+// The conv layer (block, conv) names and its index in net->convs, which is its entry in the device tables; `who`
+// prefixes the refusals.
 static int find_conv(const dirb200_net* net, int block, int conv, const char* who, const ConvLayer** cv_out,
                      int* entry_out) {
   DIRB_CHECK_ARG(block >= -1 && block < (int)net->blocks.size(), "%s: bad block %d", who, block);
   DIRB_CHECK_ARG(conv >= 0 && conv <= (block < 0 ? 0 : 3), "%s: bad conv %d", who, conv);
-  // the reduction table holds the stem, then every block's c1, c2 [, c3] [, ds] in block order (build())
-  int entry = 0;
-  const ConvLayer* cv = &net->stem;
+  int entry = 0;   // the stem
   if (block >= 0) {
     const Block& B = net->blocks[block];
     DIRB_CHECK_ARG(conv < 3 || B.has_ds, "%s: block %d has no downsample", who, block);
     DIRB_CHECK_ARG(conv != 2 || !B.basic, "%s: block %d is a basic block, it has no conv3", who, block);
-    entry = 1;
-    for (int b = 0; b < block; ++b) entry += (net->blocks[b].basic ? 2 : 3) + (net->blocks[b].has_ds ? 1 : 0);
-    entry += conv == 3 && B.basic ? 2 : conv;
-    const ConvLayer* convs[4] = {&B.c1, &B.c2, &B.c3, &B.ds};
-    cv = convs[conv];
+    entry = B.first_conv + (conv == 3 && B.basic ? 2 : conv);
   }
-  *cv_out = cv;
+  *cv_out = net->convs[entry];
   *entry_out = entry;
   return DIRB200_OK;
 }
@@ -1038,12 +989,8 @@ int dirb200_resnet_peek_conv(dirb200_net* net, int block, int conv, dirb200_conv
   out->scale = cv->bn.scale;
   out->shift = cv->bn.shift;
   out->w_off = (int64_t)cv->w_off;
-  if (cv->stem) {
-    out->cout = cv->s.cout; out->cin = 3; out->kh = 7; out->kw = 7; out->stride = 2; out->pad = 3;
-  } else {
-    out->cout = cv->s.cout; out->cin = cv->s.cin; out->kh = cv->s.kh; out->kw = cv->s.kw; out->stride = cv->s.stride;
-    out->pad = cv->s.pad;
-  }
+  const ConvShape& r = cv->ref;
+  out->cout = r.cout; out->cin = r.cin; out->kh = r.kh; out->kw = r.kw; out->stride = r.stride; out->pad = r.pad;
   out->stem = cv->stem ? 1 : 0;
   out->splits = d.splits;
   return DIRB200_OK;

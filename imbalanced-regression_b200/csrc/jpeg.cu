@@ -11,7 +11,8 @@
 //   entropy   one thread per restart interval: stuffed 0xFF00 removed on the fly, DC prediction restarting at each
 //             interval, de-zigzagged int16 coefficients (libjpeg's JCOEF).  Anomalies set the image's status;
 //   idct      one thread per 8 x 8 block: dequantisation and jidctint.c's JDCT_ISLOW (CONST_BITS 13, PASS1_BITS 2)
-//             with its range-limit table, index masked with 0x3FF;
+//             with its range-limit table, index masked with 0x3FF.  A block whose values leave the range in which
+//             libjpeg-turbo's 16-bit SIMD IDCT gives the same result sets the image's status;
 //   colour    one thread per output pixel: libjpeg-turbo's fancy h2v1 / h2v2 triangle upsampling over the chroma's
 //             downsampled width (edge rows repeated as libjpeg's context rows are), jdcolor.c's YCbCr -> RGB with
 //             SCALEBITS 16; grayscale is replicated to three channels as convert('RGB') does.
@@ -54,6 +55,7 @@ constexpr int kBadCode = 2;        // a code that is not in the Huffman table
 constexpr int kOverrun = 4;        // entropy-coded data ran out (the decode consumed bits past a marker / range end)
 constexpr int kTooMany = 8;        // a coefficient past position 63 of a block
 constexpr int kWorkspace = 16;     // the workspace does not hold the batch
+constexpr int kIdctRange = 32;     // a block outside the range in which libjpeg-turbo's SIMD and C IDCTs agree
 
 // ---------------------------------------------------------------------------------------------- shared descriptor rules
 __host__ __device__ inline int comp_blocks_w(const Desc& d, int c) { return d.ncomp == 1 ? d.mcus_x : d.mcus_x * d.comp_h[c]; }
@@ -475,18 +477,38 @@ __host__ __device__ __forceinline__ void islow_1d(const int32_t in[8], int32_t o
   out[4] = (tmp13 - tmp0 + add) >> shift;
 }
 
+// Range in which every IDCT of libjpeg-turbo gives jidctint.c's 32-bit C result.  Its x86-64 SIMD islow dequantises
+// and adds pairs of values in 16-bit lanes, saturates (packssdw) the pass-1 results, and saturates its output where the
+// C range limit wraps (index & 0x3FF).  The coefficients of an 8-bit image's blocks stay far inside this range.
+constexpr int32_t kIdctInMax = 16383;        // |dequantised value|: a sum of two fits in int16
+constexpr int32_t kIdctMidMax = 16383;       // |pass-1 result|: likewise
+constexpr int32_t kIdctOutMin = -512, kIdctOutMax = 511;   // pass-2 result: C's wrapped index equals saturation
+
+__host__ __device__ __forceinline__ bool outside(int32_t v, int32_t lo, int32_t hi) {
+  return static_cast<uint32_t>(v - lo) > static_cast<uint32_t>(hi - lo);
+}
+
 // jpeg_idct_islow of one block: coefficients natural order, quant natural order -> 8 x 8 samples (row stride `ld`).
-// The all-zero-AC shortcuts of the reference give the same values as the full pass, so they are not restated.
-__host__ __device__ __forceinline__ void idct_islow(const int16_t* co, const uint16_t* q, uint8_t* out, int64_t ld) {
+// Returns false when a value leaves the range above: libjpeg-turbo's SIMD and C IDCTs may then disagree (the C code's
+// zero-AC shortcuts too: they equal the full pass only while the << CONST_BITS of the full pass does not overflow,
+// which the range keeps), so the block's pixels are not Pillow's.
+__host__ __device__ __forceinline__ bool idct_islow(const int16_t* co, const uint16_t* q, uint8_t* out, int64_t ld) {
   int32_t ws[64];
+  bool bad = false;
 #pragma unroll
   for (int col = 0; col < 8; ++col) {
     int32_t in[8], o[8];
 #pragma unroll
-    for (int r = 0; r < 8; ++r) in[r] = static_cast<int32_t>(co[r * 8 + col]) * static_cast<int32_t>(static_cast<int16_t>(q[r * 8 + col]));
+    for (int r = 0; r < 8; ++r) {
+      in[r] = static_cast<int32_t>(co[r * 8 + col]) * static_cast<int32_t>(static_cast<int16_t>(q[r * 8 + col]));
+      bad |= outside(in[r], -kIdctInMax, kIdctInMax);
+    }
     islow_1d(in, o, kConstBits - kPass1Bits, 1 << (kConstBits - kPass1Bits - 1));
 #pragma unroll
-    for (int r = 0; r < 8; ++r) ws[r * 8 + col] = o[r];
+    for (int r = 0; r < 8; ++r) {
+      ws[r * 8 + col] = o[r];
+      bad |= outside(o[r], -kIdctMidMax, kIdctMidMax);
+    }
   }
   constexpr int kShift2 = kConstBits + kPass1Bits + 3;
 #pragma unroll
@@ -495,15 +517,19 @@ __host__ __device__ __forceinline__ void idct_islow(const int16_t* co, const uin
     islow_1d(ws + r * 8, o, kShift2, 1 << (kShift2 - 1));
     uint8_t* dst = out + r * ld;
 #pragma unroll
-    for (int c = 0; c < 8; ++c) dst[c] = idct_limit(o[c]);
+    for (int c = 0; c < 8; ++c) {
+      dst[c] = idct_limit(o[c]);
+      bad |= outside(o[c], kIdctOutMin, kIdctOutMax);
+    }
   }
+  return !bad;
 }
 
 constexpr int kIdctGx = 64;
 
 __global__ void __launch_bounds__(128)
 jpeg_idct_kernel(const Desc* __restrict__ descs, const ImgPlan* __restrict__ plans, const int16_t* __restrict__ coef,
-                 uint8_t* __restrict__ planes) {
+                 uint8_t* __restrict__ planes, int32_t* __restrict__ status) {
   const int b = blockIdx.y;
   const ImgPlan plan = plans[b];
   if (!plan.ok) return;
@@ -532,7 +558,7 @@ jpeg_idct_kernel(const Desc* __restrict__ descs, const ImgPlan* __restrict__ pla
     for (int i = 0; i < 32; ++i) reinterpret_cast<uint32_t*>(q)[i] = qs[i];
     const int64_t ld = static_cast<int64_t>(bwc) * 8;
     uint8_t* dst = planes + (plan.plane + first * 64) + (static_cast<int64_t>(by) * 8) * ld + bx * 8;
-    idct_islow(co, q, dst, ld);
+    if (!idct_islow(co, q, dst, ld)) atomicOr(status + b, kIdctRange);
   }
 }
 
@@ -1049,7 +1075,7 @@ int dirb200_jpeg_decode(const uint8_t* data, const int64_t* offsets, const dirb2
   DIRB_LAUNCHED();
   jpeg_entropy_kernel<<<dim3(kEntropyGx, n), 32, 0, st>>>(data, offsets, descs, intervals, plans, tabs, coef, status);
   DIRB_LAUNCHED();
-  jpeg_idct_kernel<<<dim3(kIdctGx, n), 128, 0, st>>>(descs, plans, coef, planes);
+  jpeg_idct_kernel<<<dim3(kIdctGx, n), 128, 0, st>>>(descs, plans, coef, planes, status);
   DIRB_LAUNCHED();
   jpeg_colour_kernel<<<dim3(kColourGx, n), 256, 0, st>>>(descs, plans, planes, rgb_out, rgb_offsets);
   DIRB_LAUNCHED();

@@ -275,7 +275,8 @@ int dirb200_jpeg_parse(const uint8_t* data_host, int64_t nbytes, dirb200_jpeg_de
  * at [rgb_offsets[b], rgb_offsets[b + 1]) (int64 [n + 1]), which must hold height * width * 3 bytes.
  * status int32 [n] (written): 0, or nonzero where the device found an anomaly -- a descriptor outside the supported
  * set or its byte range, a code not in a Huffman table, entropy data running out, more than 64 coefficients in a
- * block -- or the workspace is too small.  Such an image's pixels are unspecified: decode it on the host.  No kernel
+ * block, a block whose dequantised values or IDCT results leave the range in which libjpeg-turbo's 16-bit SIMD IDCT
+ * and its 32-bit C IDCT agree -- or the workspace is too small.  Such an image's pixels are unspecified: decode it on the host.  No kernel
  * reads outside an image's byte range or writes outside its output slice.  Stages: Huffman tables, entropy decode
  * (one thread per restart interval), dequantisation + libjpeg's JDCT_ISLOW IDCT, libjpeg-turbo's fancy upsampling and
  * YCbCr -> RGB.  The workspace holds the int16 coefficients and the component planes (192 bytes per 8 x 8 block). */

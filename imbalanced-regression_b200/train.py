@@ -38,8 +38,24 @@ from parallel import DataParallel, ShardSampler, is_distributed
 print = logging.info
 
 
+# The defaults that agedb-dir/train.py and imdb-wiki-dir/train.py do not share (lines 29, 35 and 40 of each): the
+# parser takes them from the script of the --dataset given, so `--dataset imdb_wiki` trains with IMDB-WIKI-DIR's LDS /
+# FDS windows and FDS buckets from age 0.  Flags given explicitly still win.
+DATASET_DEFAULTS = {'agedb': dict(lds_ks=9, fds_ks=9, bucket_start=3),
+                    'imdb_wiki': dict(lds_ks=5, fds_ks=5, bucket_start=0)}
+
+
+class _Parser(argparse.ArgumentParser):
+    def parse_known_args(self, args=None, namespace=None):
+        pre = argparse.ArgumentParser(add_help=False, allow_abbrev=False)
+        pre.add_argument('--dataset', type=str, default='agedb')
+        dataset = pre.parse_known_args(args)[0].dataset
+        self.set_defaults(**DATASET_DEFAULTS.get(dataset, DATASET_DEFAULTS['agedb']))
+        return super().parse_known_args(args, namespace)
+
+
 def build_parser():
-    p = argparse.ArgumentParser(formatter_class=argparse.ArgumentDefaultsHelpFormatter)
+    p = _Parser(formatter_class=argparse.ArgumentDefaultsHelpFormatter)
     p.add_argument('--lds', action='store_true', default=False, help='whether to enable LDS')
     p.add_argument('--lds_kernel', type=str, default='gaussian', choices=['gaussian', 'triang', 'laplace'])
     p.add_argument('--lds_ks', type=int, default=9, help='LDS kernel size: should be odd number')
@@ -216,7 +232,9 @@ def shot_metrics(preds, labels, train_labels, many_shot_thr=100, low_shot_thr=20
         raise TypeError(f'Type ({type(preds)}) of predictions not supported')
     p, l, t = as_dev(preds), as_dev(labels), as_dev(train_labels)
     assert p.numel() == l.numel()
-    nbins = int(max(float(t.max()) if t.numel() else 0.0, float(l.max()) if l.numel() else 0.0, 0.0)) + 2
+    # NaN training labels are skipped by the histogram (a NaN max would not convert to a bin count)
+    top = lambda x: float(torch.nan_to_num(x, nan=0.0).max()) if x.numel() else 0.0
+    nbins = int(max(top(t), top(l), 0.0)) + 2
     hist = torch.zeros(nbins, dtype=torch.int64, device=dev)
     _lib.call("dirb200_int_label_histogram", _lib.ptr(t), t.numel(), nbins, _lib.ptr(hist), _lib.stream_ptr())
     out = torch.empty(4, 4, dtype=torch.float64, device=dev)
@@ -260,6 +278,8 @@ def validate(val_loader, model, train_labels=None, prefix='Val'):
 
 
 def main(argv=None):
+    """Trains, then tests the best checkpoint; returns the test split's (MSE, L1, G-Mean).  With --evaluate: only
+    the test pass of the --resume checkpoint, same return."""
     args, _ = build_parser().parse_known_args(argv)
     args.device_transform = args.device_transform or args.device_decode
     args.start_epoch, args.best_loss = 0, 1e5
@@ -321,8 +341,8 @@ def main(argv=None):
         assert args.resume, 'Specify a trained model using [args.resume]'
         checkpoint = torch.load(args.resume)
         model.load_state_dict(checkpoint['state_dict'], strict=False)
-        validate(test_loader, model, train_labels=train_labels, prefix='Test')
-        return
+        print(f"===> Checkpoint '{args.resume}' loaded (epoch [{checkpoint['epoch']}]), testing...")
+        return validate(test_loader, model, train_labels=train_labels, prefix='Test')
 
     if args.retrain_fc:
         assert args.reweight != 'none' and args.pretrained
@@ -354,6 +374,7 @@ def main(argv=None):
         metric = val_mse if args.loss == 'mse' else val_l1
         is_best = metric < args.best_loss
         args.best_loss = min(metric, args.best_loss)
+        print(f"Best {'L1' if 'l1' in args.loss else 'MSE'} Loss: {args.best_loss:.3f}")
         if rank == 0:
             save_checkpoint(args, {'epoch': epoch + 1, 'model': args.model, 'best_loss': args.best_loss,
                                    'state_dict': model.state_dict(), 'optimizer': optimizer.state_dict()}, is_best)
@@ -363,8 +384,20 @@ def main(argv=None):
             st = take_device_decode_stats()
             print(f"Epoch #{epoch}: images decoded on the device {st['device']}, flagged by it and decoded by Pillow "
                   f"{st['flagged']}, outside its supported set (decoded by Pillow in the loader) {st['host']}")
+
+    # test with the best checkpoint (agedb-dir/train.py:224-231); only rank 0 writes it
+    print("=" * 120)
+    print("Test best model on testset...")
+    if is_distributed():
+        torch.distributed.barrier()
+    checkpoint = torch.load(os.path.join(args.store_root, args.store_name, 'ckpt.best.pth.tar'), map_location='cuda')
+    model.load_state_dict(checkpoint['state_dict'])
+    print(f"Loaded best model, epoch {checkpoint['epoch']}, best val loss {checkpoint['best_loss']:.4f}")
+    test_mse, test_l1, test_gmean = validate(test_loader, model, train_labels=train_labels, prefix='Test')
+    print(f"Test loss: MSE [{test_mse:.4f}], L1 [{test_l1:.4f}], G-Mean [{test_gmean:.4f}]\nDone")
     if is_distributed():
         torch.distributed.destroy_process_group()
+    return test_mse, test_l1, test_gmean
 
 
 if __name__ == '__main__':

@@ -329,7 +329,8 @@ int dirb200_int_label_histogram(const float* labels, int64_t n, int nbins, int64
  * :286-335).  A sample is "many"-shot when the training count of its label value is > many_shot_thr, "low" when
  * it is < low_shot_thr (label values absent from training or not integer valued count 0), else "median".
  * out16 (double[4][4], OVERWRITTEN): rows = overall, many, median, low; columns = count, sum (pred-label)^2,
- * sum |pred-label|, sum log|pred-label|  ->  mse = c1/c0, l1 = c2/c0, gmean = exp(c3/c0). */
+ * sum |pred-label|, sum log|pred-label|  ->  mse = c1/c0, l1 = c2/c0, gmean = exp(c3/c0).  One CTA sums in a fixed
+ * order (no floating-point atomics): identical calls give identical bits. */
 int dirb200_shot_metrics(const float* preds, const float* labels, int64_t n, const int64_t* train_hist, int nbins,
                          int many_shot_thr, int low_shot_thr, double* out16, void* stream);
 
